@@ -1,6 +1,7 @@
 """bench.py — headline benchmark of the DiffBIR hot path (see BASELINE.json).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload 512|tiled2048]
+                    [--dump-outputs DIR]
 
 A "step" is one full restoration of one synthetic image per GPU through SwinIRPipeline: SwinIR
 stage 1 -> VAE encode + CLIP -> 50-step spaced sampler (cfg 4.0, ControlNet + UNet, batched
@@ -9,8 +10,8 @@ cond/uncond) -> VAE decode -> colour fix -> uint8.  Random-init SD-2.1 / SwinIR 
 
   value : MPix/s with the uint8 input already resident in HBM (CUDA-event time, max over ranks)
   e2e   : the same through the public API Pipeline.run(host uint8) -> host uint8 (H2D + D2H inside)
-  roofline : tcgen05 GEMM/conv kernel family — algorithmic FLOPs of every launch of one
-             ControlNet+UNet forward / CUDA-event time of those launches, vs the measured bf16 peak
+  roofline : wgmma GEMM/conv kernel family — algorithmic FLOPs of every launch of one
+             ControlNet+UNet forward / CUDA-event time of those launches, vs the dense bf16 peak
   cpu_baseline : the fp32 oracle port of the reference on the host cores, bounded sample
                  (1 of 50 sampler steps; SwinIR, VAE encode/decode once), extrapolated.
 
@@ -27,7 +28,13 @@ cond/uncond) -> VAE decode -> colour fix -> uint8.  Random-init SD-2.1 / SwinIR 
 
 Multi-GPU (torchrun, one rank per GPU): the 512x512 workload has no tiles, so ranks are
 independent replicas (weak scaling, no collective); --workload tiled2048 makes the tiled run the
-headline `value` instead (strong scaling).
+headline `value` instead (strong scaling); --steps then sets the number of timed tiled images
+(--tiled-images does otherwise).
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step of the headline path
+returned (the restored uint8 NHWC image) as float32: DIR/restored_512.npy, or DIR/restored_2048_tiled.npy
+with --workload tiled2048. Inputs, weights and noise are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import json
@@ -35,6 +42,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 from pathlib import Path
@@ -51,7 +59,7 @@ def log(*a):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -93,13 +101,15 @@ class ClockSampler:
 
 
 def measured_peaks():
-    """(sustained bf16 TFLOP/s, burst bf16 TFLOP/s, HBM GB/s, source)"""
+    """(sustained bf16 TFLOP/s, burst bf16 TFLOP/s, HBM GB/s, source). Without a measurement file: NVIDIA's
+    H100 SXM data sheet (dense bf16 989 TFLOP/s, HBM3 3.35 TB/s, for a card allowed 700 W) -- an upper
+    bound, not a rate this machine has been shown to reach."""
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return (d.get("bf16_tflops_sustained", 1400.0), d.get("bf16_tflops", 1590.0), d.get("hbm_gbs", 6650.0),
+        return (d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0),
                 "measured (MEASURED_PEAKS.json)")
-    return 1400.0, 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 989.0, 3350.0, "H100 SXM data sheet (dense bf16, 700 W)"
 
 
 def host_threads() -> int:
@@ -404,8 +414,15 @@ def leg_main(name: str):
         raise SystemExit(f"unknown leg {name}")
 
 
+def dump(dir_name: str, name: str, out):
+    """--dump-outputs: one array a caller of the timed path received, as float32 .npy"""
+    import numpy as np
+    d = Path(dir_name)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / f"{name}.npy", out.float().cpu().numpy())
+
+
 def run_ours(args):
-    import numpy as np  # noqa: F401
     import torch
     from diffbir_b200 import lib
     from diffbir_b200.sampler import sampler as sampler_mod
@@ -424,6 +441,7 @@ def run_ours(args):
     lib.load()
     dog = Watchdog(rank)
     headline_tiled = args.workload == "tiled2048"
+    n_tiled = args.steps if headline_tiled else args.tiled_images      # timed tiled 2048^2 images
     t_build = time.time()
     pipe = build_synthetic_pipeline(dev, seed=1234)
     log(f"[rank {rank}] pipeline built in {time.time() - t_build:.1f}s")
@@ -465,11 +483,13 @@ def run_ours(args):
     torch.cuda.nvtx.range_push("dbir_timed")      # ncu --nvtx --nvtx-include "dbir_timed/" profiles exactly this region
     e0.record()
     for _ in range(args.steps):
-        one(True)
+        res = one(True)
     e1.record()
     torch.cuda.nvtx.range_pop()
     barrier()
     dev_ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0 and not headline_tiled:
+        dump(args.dump_outputs, "restored_512", res)
     launches = lib.launches() - n0
     # end-to-end through the public API (pinned host uint8 in, host uint8 out)
     barrier()
@@ -501,7 +521,7 @@ def run_ours(args):
         "config": {
             "workload": wl_512, "images_per_gpu_per_step": 1, "sampler_steps": SAMPLER_STEPS,
             "parallelism": "independent replicas, no collective (the sharded path with a collective is the tiled2048 block)",
-            "l2": "no flush needed: each forward streams 2.6 GB of weights >> 126 MB L2",
+            "l2": "no flush needed: each forward streams 2.6 GB of weights >> 50 MB L2",
         },
         "e2e": {"value": e2e_512, "unit": "MPix/s", "h2d_bytes_per_step": int(lq.nbytes), "d2h_bytes_per_step": int(out.nbytes),
                 "ms_per_step": e2e_ms / args.steps},
@@ -546,22 +566,24 @@ def run_ours(args):
         sampler_mod.Sampler.time_collective = True
         pipe.marks = []
         t_ms, t_e2e_ms = [], []
-        for _ in range(args.tiled_images):
+        for _ in range(n_tiled):
             barrier()
             a0, a1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             torch.manual_seed(231)
             a0.record()
-            pipe.run_device(lq_t_dev, **tkw)
+            res_t = pipe.run_device(lq_t_dev, **tkw)
             a1.record()
             barrier()
             t_ms.append(a0.elapsed_time(a1))
+        if args.dump_outputs and rank == 0 and headline_tiled:
+            dump(args.dump_outputs, "restored_2048_tiled", res_t)
         tphases = pipe.phases_ms()
         smp = pipe.last_sampler
         ag = [a.elapsed_time(b) for a, b in smp.last_stats.get("allgather_events", [])]
         stats = dict(smp.last_stats)
         pipe.marks = None
         sampler_mod.Sampler.time_collective = False
-        for _ in range(args.tiled_images):
+        for _ in range(n_tiled):
             barrier()
             w0 = time.perf_counter()
             torch.manual_seed(231)
@@ -576,9 +598,9 @@ def run_ours(args):
         counts[rank] = stats.get("units_this_rank", 0)
         if world > 1:
             dist.all_reduce(counts)
-        mp = args.tiled_images * 2048 * 2048 / 1e6
-        tiled = {"value": mp / (t_total / 1e3), "unit": "MPix/s", "scaling": "strong", "images": args.tiled_images,
-                 "ms_per_image": t_total / args.tiled_images,
+        mp = n_tiled * 2048 * 2048 / 1e6
+        tiled = {"value": mp / (t_total / 1e3), "unit": "MPix/s", "scaling": "strong", "images": n_tiled,
+                 "ms_per_image": t_total / n_tiled,
                  "e2e": {"value": mp / (t_e2e_total / 1e3), "unit": "MPix/s", "h2d_bytes_per_step": int(lq_t.nbytes),
                          "d2h_bytes_per_step": int(out_t.nbytes)},
                  "tiles": int(stats.get("tiles", 0)), "tile_forwards_per_rank": [int(c) for c in counts.tolist()],
@@ -658,22 +680,12 @@ def run_ours(args):
     gf, gms, gn = fam[gname]
     achieved = gf / (gms * 1e-3) / 1e12
     forward_ms = sum(v[1] for v in fam.values())
-    traffic = None
-    for cand in ("r02_ncu_full_summary.json", "r01_ncu_full_summary.json"):
-        tpath = ROOT / "profiles" / cand
-        if tpath.exists():       # dram bytes (read + write) per launch from the committed `ncu --set full` capture
-            rows = [r for r in json.loads(tpath.read_text()) if "gemm_tc_kernel" in r["kernel"]]
-            if rows:
-                traffic = {"dram_bytes_per_launch_mean": sum(r["dram_bytes"] for r in rows) / len(rows),
-                           "l2_to_sm_bytes_per_launch_mean": sum(r["l2_to_sm_bytes"] for r in rows) / len(rows),
-                           "launches": len(rows), "source": f"profiles/{cand}"}
-                break
     att = fam.get("attention (attn_fwd_kernel)", [0, 1, 0])
     roof = {"bound": "tensor", "kernel": gname, "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s",
             "frac": achieved / peak_tf, "frac_of_burst_peak": achieved / peak_burst, "peak_burst": peak_burst,
-            "peak_note": "frac = achieved / sustained cuBLAS bf16 peak (the family is timed inside a long step); "
+            "peak_note": "frac = achieved / sustained bf16 peak (the family is timed inside a long step); "
                          "frac_of_burst_peak uses the isolated-kernel figure",
-            "traffic": traffic, "peak_source": peak_src,
+            "peak_source": peak_src,
             "launches_per_forward": gn, "algorithmic_gflop_per_forward": gf / 1e9,
             "kernel_ms_per_forward": gms,
             "attention": {"achieved": att[0] / (att[1] * 1e-3) / 1e12, "frac": att[0] / (att[1] * 1e-3) / 1e12 / peak_tf,
@@ -688,13 +700,12 @@ def run_ours(args):
             "forwards_per_replay": 14, "gemm_tflops": tg[0] / (tg[1] * 1e-3) / 1e12, "gemm_frac": tg[0] / (tg[1] * 1e-3) / 1e12 / peak_tf,
             "gemm_ms": tg[1], "attention_tflops": ta[0] / (ta[1] * 1e-3) / 1e12, "attention_frac": ta[0] / (ta[1] * 1e-3) / 1e12 / peak_tf,
             "attention_ms": ta[1], "note": "same kernel families at the per-rank batch of the 8-GPU tiled-2048 run (batch-invariant plans)"}
-    prof_dir = ROOT / "gpurun_out"
-    prof_dir.mkdir(exist_ok=True)
-    with open(prof_dir / "kernel_census.csv", "w") as f:
+    census = Path(tempfile.gettempdir()) / f"dbir_kernel_census_{os.getpid()}.csv"     # never inside the tree
+    with open(census, "w") as f:
         f.write("kind,shape,launches,gflop,ms,tflops\n")
         for k, (fl, ms, n) in sorted(shapes.items(), key=lambda kv: -kv[1][1]):
             f.write(f"{k[0]},{'x'.join(map(str, k[1:]))},{n},{fl / 1e9:.2f},{ms:.4f},{fl / (ms * 1e-3) / 1e12 if ms > 0 else 0:.1f}\n")
-    log("[rank 0] kernel census done")
+    log(f"[rank 0] kernel census done: per-shape table in {census}")
     line["roofline"], dog.phase = roof, "baselines"
     # ---- baselines on the same box, N = 1 only ------------------------------------------------
     cpu = gpu_base = None
@@ -711,7 +722,7 @@ def run_ours(args):
     if headline_tiled and tiled is not None:
         line.update(metric="MPix/s end-to-end 50-step restore, tiled 2048px", value=tiled["value"],
                     ms_per_step=tiled["ms_per_image"], scaling="strong", e2e=tiled["e2e"],
-                    steps=args.tiled_images)
+                    steps=n_tiled)
         line["config"]["workload"] = tiled["workload"]
         line["config"]["parallelism"] = "tiles sharded round-robin + all-gather"
         line["replicas512"] = {"value": value_512, "e2e": e2e_512, "ms_per_step": dev_ms / args.steps}
@@ -732,8 +743,18 @@ def main():
     ap.add_argument("--no-v21", action="store_true", help="skip the v2.1 1024^2 batch-4 block")
     ap.add_argument("--no-batch4", action="store_true", help="skip the 4-images-per-call 512^2 block")
     ap.add_argument("--tiled-images", type=int, default=1)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's output of the headline path to DIR (float32 .npy)")
     ap.add_argument("--leg", default="", help=argparse.SUPPRESS)      # internal: one baseline leg in a child process
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.tiled_images < 1:
+        ap.error("--tiled-images must be at least 1")
+    if args.workload == "tiled2048" and args.no_tiled:
+        ap.error("--workload tiled2048 times the tiled block: it cannot be combined with --no-tiled")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs needs --impl ours: the reference arm times a bounded CPU sample and returns no image")
     if args.leg:
         leg_main(args.leg)
     elif args.impl == "reference":

@@ -6,7 +6,7 @@ def unsupported(name: str, reference: str, instead: str):
 
     def __init__(self, *args, **kwargs):
         raise NotImplementedError(
-            f"diffbir.{name} ({reference}) is not on the B200 hot path (SURVEY.md 8f); {instead}")
+            f"diffbir.{name} ({reference}) is not on the H100 hot path (SURVEY.md 8f); {instead}")
 
     return type(name, (), {"__init__": __init__, "__doc__": f"Not built: {reference}. {instead}",
                            "__module__": "diffbir"})

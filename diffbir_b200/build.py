@@ -1,12 +1,11 @@
-"""In-tree build of libdiffbir_b200.so (sm_100a only; nvcc cross-compiles without a GPU).
+"""In-tree build of libdiffbir_b200.so (sm_90a only; nvcc cross-compiles without a GPU).
 
     python -m diffbir_b200.build [--bf16] [--force] [-DNAME ...]
 
-Extra -D switches (also from $DBIR_BUILD_DEFS) select compile-time experiments, e.g.
--DDBIR_DEBUG_PROBES -DDBIR_ATTN_PROBE (calibration probes: tools/gpu_mma_rate.py, tools/gpu_attn_probe.py).
+Extra -D switches (also from $DBIR_BUILD_DEFS) select compile-time experiments.
 
 Objects go to diffbir_b200/csrc/_build/, the library to diffbir_b200/libdiffbir_b200.so
-(git-ignored; it travels to the GPU box with the gpurun snapshot). --bf16 builds the bf16-operand
+(git-ignored). --bf16 builds the bf16-operand
 variant into csrc/_build_bf16/ and libdiffbir_b200_bf16.so (loaded when DBIR_OPERANDS=bf16).
 """
 from __future__ import annotations
@@ -23,7 +22,7 @@ CSRC = HERE / "csrc"
 OUT = HERE / "libdiffbir_b200.so"
 OUT_BF16 = HERE / "libdiffbir_b200_bf16.so"      # -DDBIR_OPERAND_BF16 variant, selected with DBIR_OPERANDS=bf16
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
          "-Xptxas", "-v"]
 

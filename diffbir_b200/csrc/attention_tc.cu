@@ -1,21 +1,19 @@
-// Flash attention for head_dim 64 on tcgen05 / TMEM (self- and cross-attention of the
-// SpatialTransformer: reference attention.py:189-216 `F.scaled_dot_product_attention`,
-// with the head split/merge copies of :196-214 folded into TMA coordinates).
+// Flash attention for head_dim 64 on wgmma (self- and cross-attention of the SpatialTransformer:
+// reference attention.py:189-216 `F.scaled_dot_product_attention`, with the head split/merge copies
+// of :196-214 folded into TMA coordinates).
 //
 //   O[b, i, h*64:(h+1)*64] = softmax_j(Q_h[i] . K_h[j] / 8) V_h[j]
 //
 // Q/K/V are 16-bit matrices [B, S, ld] (any row stride / column offset, e.g. slices of a fused
 // QKV projection). One CTA = one (128-query tile, head, batch), keys in steps of 64:
-//   warp 0    TMA producer  (Q once, K/V steps of 64 keys, 4 stages)
-//   warp 1    MMA issuer    S(j) = Q K(j)^T -> TMEM S[j % 2] (64 columns each), O += P(j) V(j)
-//   warps 2-5 softmax       thread == query row: 64 scores into registers, online softmax in fp32
-//                           with exp2, P(j) (16-bit) -> swizzled smem buffer j % 2
-// S and P are double buffered and the issuer runs one step ahead (QK(j+1) is in flight while the
-// softmax warps work on step j, PV(j) starts as soon as P(j) lands), so the softmax warps - the
-// MUFU-bound part - rarely wait for the tensor pipe. The running max is only raised when a row
-// max grows by more than 2^8 (any reference point is a valid softmax shift; P stays < 2^8 and l
-// carries the same scale), so the fp32 O accumulator in TMEM is rescaled (tcgen05.ld/st) rarely.
-// Two CTAs are resident per SM (112 KB smem, 256 TMEM columns each).
+//   warp 8      TMA producer (Q once per tile, K/V steps of 64 keys, 4 stages)
+//   warps 0-7   two consumer warpgroups, 64 query rows each: S = Q K^T (wgmma, both operands in
+//               shared memory, S in registers), online softmax in fp32 with exp2 on the accumulator
+//               fragment (row reductions over the 4 lanes that share a row), then O += P V with P
+//               taken from registers (16-bit) and V read transposed from shared memory.
+// The running max is only raised when a row max grows by more than 2^8 (any reference point is a
+// valid softmax shift; P stays < 2^8 and l carries the same scale), so O is rescaled rarely.
+// Two CTAs are resident per SM (80 KB shared memory each).
 #include "common.cuh"
 #include "../../include/diffbir_b200.h"
 #include <stdlib.h>
@@ -28,15 +26,9 @@ constexpr int DH = 64;
 constexpr int KV_STAGES = 4;
 constexpr int Q_BYTES = TQ * DH * 2;       // 16 KB
 constexpr int KV_BYTES = TK * DH * 2;      // 8 KB per K or V step
-constexpr int P_BYTES = TQ * TK * 2;       // 16 KB
-constexpr uint32_t TMEM_COLS = 256;
-constexpr uint32_t TM_S = 0, TM_O = 128;   // S[0] @0, S[1] @64, O @128
+constexpr int ATTN_THREADS = 288;          // two consumer warpgroups + the producer warp
+constexpr int CTAS_PER_SM = 2;
 constexpr float RESCALE_LOG2 = 8.0f;
-#ifdef DBIR_ATTN_PROBE
-constexpr bool PROBE = true;     // clock64 phase sums for tools/gpu_attn_probe.py
-#else
-constexpr bool PROBE = false;
-#endif
 struct AttnParams {
   int sq, skv, heads;
   void* out;
@@ -51,22 +43,17 @@ struct AttnParams {
   long long total_steps;
   unsigned int* tickets;   // [tiles], zero on entry, self-resetting
   float* ws;               // [tiles][parts_max][WS_ROW planes][128 rows]
-  long long* dbg;          // per-CTA clock64 sums [ctas][8] (dbir_debug_attn_stamps; needs -DDBIR_ATTN_PROBE)
 };
 constexpr int WS_ROW = DH + 2;   // O[64], m_ref, l
 
 struct __align__(8) AttnBarriers {
-  uint64_t q_full, q_empty, o_free;
+  uint64_t q_full, q_empty;
   uint64_t kv_full[KV_STAGES];
   uint64_t kv_empty[KV_STAGES];
-  uint64_t s_full[2];
-  uint64_t p_full[2];
-  uint64_t o_full[2];
-  uint32_t tmem_slot;
   uint32_t last_flag;
 };
 
-constexpr int ATTN_SMEM = Q_BYTES + 2 * KV_STAGES * KV_BYTES + 2 * P_BYTES + 256;
+constexpr int ATTN_SMEM = Q_BYTES + 2 * KV_STAGES * KV_BYTES + 256;
 
 __device__ __forceinline__ int sk_bound(const AttnParams& p, int c) {
   if (p.parts_max == 0) return c * p.n_steps;           // one whole tile per CTA
@@ -80,55 +67,46 @@ __device__ __forceinline__ int sk_owner(const AttnParams& p, int x) {
   return c;
 }
 
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
 // SK = false: one whole tile per CTA (grid == tiles), the partial-tile machinery compiles away.
 template <bool SK>
-__global__ void __launch_bounds__(192, 2)
+__global__ void __launch_bounds__(ATTN_THREADS, CTAS_PER_SM)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
                 const __grid_constant__ CUtensorMap tma_v, const AttnParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + Q_BYTES;
   uint8_t* sV = sK + KV_STAGES * KV_BYTES;
-  uint8_t* sP = sV + KV_STAGES * KV_BYTES;              // two [128 x 64] swizzled P buffers
-  AttnBarriers* bar = reinterpret_cast<AttnBarriers*>(sP + 2 * P_BYTES);
+  AttnBarriers* bar = reinterpret_cast<AttnBarriers*>(sV + KV_STAGES * KV_BYTES);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_steps = p.n_steps;
   const int g_begin = SK ? sk_bound(p, blockIdx.x) : static_cast<int>(blockIdx.x) * n_steps;
   const int g_end = SK ? sk_bound(p, blockIdx.x + 1) : g_begin + n_steps;
 
-  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) {
-    printf("dbir attention: dynamic smem base not 1024-byte aligned\n");
-    __trap();
-  }
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();   // swizzled operands need 1024-byte alignment
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tma_q); tma_prefetch_desc(&tma_k); tma_prefetch_desc(&tma_v);
-  }
-  if (warp == 1 && lane == 0) {
     mbar_init(&bar->q_full, 1);
-    mbar_init(&bar->q_empty, 1);
-    mbar_init(&bar->o_free, 128);
-    for (int s = 0; s < KV_STAGES; ++s) { mbar_init(&bar->kv_full[s], 1); mbar_init(&bar->kv_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bar->s_full[s], 1);
-      mbar_init(&bar->p_full[s], 128);
-      mbar_init(&bar->o_full[s], 1);
-    }
+    mbar_init(&bar->q_empty, 2);
+    for (int s = 0; s < KV_STAGES; ++s) { mbar_init(&bar->kv_full[s], 1); mbar_init(&bar->kv_empty[s], 2); }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(&bar->tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bar->tmem_slot;
   pdl_trigger();
   pdl_wait();
 
   // Every role walks the same list of segments (tile, key steps [a, e)) of this CTA's range; `it`
   // counts the CTA's key steps across segments and selects pipeline stages / barrier phases.
-  // Warps 0 / 1 run warp-uniform loops and elect one lane per TMA / MMA / commit: inside a plain
-  // `if (lane == 0)` region the compiler serialises every such instruction through a per-lane loop.
-  if (warp == 0) {
+  if (warp == 8) {
     int it = 0, seg = 0;
     for (int g = g_begin; g < g_end; ++seg) {
       const int tile = g / n_steps;
@@ -154,268 +132,166 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant
       }
       g += e - a;
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc_s = umma_idesc(TK, 0, 0);   // S[128 x 64]: Q, K both K-major
-    constexpr uint32_t idesc_o = umma_idesc(DH, 0, 1);   // O[128 x 64]: P K-major, V MN-major
-    const uint64_t q_desc = umma_desc_sw128(smem_u32(sQ));
-    const uint64_t p_desc0 = umma_desc_sw128(smem_u32(sP));
-    const uint64_t k_desc0 = umma_desc_sw128(smem_u32(sK));
-    const uint64_t v_desc0 = umma_desc_sw128(smem_u32(sV));
-    // S = Q K^T for the CTA's step `i` into S buffer i % 2; descriptor start addresses advance in
-    // 16-byte units. `last` = last QK of the tile: Q may be replaced once it retires.
-    auto issue_qk = [&](int i, bool last) {
-      const int st = i % KV_STAGES;
-      mbar_wait(&bar->kv_full[st], (i / KV_STAGES) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t k_desc = k_desc0 + static_cast<uint64_t>((st * KV_BYTES) >> 4);
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k)
-          umma_f16(tmem_base + TM_S + (i & 1) * TK, q_desc + 2 * k, k_desc + 2 * k, idesc_s, k != 0 ? 1u : 0u);
-        umma_commit(&bar->s_full[i & 1]);
-        if (last) umma_commit(&bar->q_empty);
-      }
-      __syncwarp();
-    };
-    int it = 0, seg = 0;
-    long long d_wp = 0;
-    for (int g = g_begin; g < g_end; ++seg) {
-      const int tile = g / n_steps;
-      const int a = g - tile * n_steps;
-      const int e = min(g_end, (tile + 1) * n_steps) - tile * n_steps;
-      const int len = e - a;
-      mbar_wait(&bar->q_full, seg & 1);
-      issue_qk(it, len == 1);
-      if (len > 1) issue_qk(it + 1, len == 2);
-      for (int jl = 0; jl < len; ++jl, ++it) {
-        const int st = it % KV_STAGES;
-        // P (written by the softmax warps, which are then also done reading S) x V
-        long long cp0 = 0;
-        if (PROBE && p.dbg) cp0 = clock64();
-        mbar_wait(&bar->p_full[it & 1], (it >> 1) & 1);
-        if (PROBE && p.dbg) d_wp += clock64() - cp0;
-        // the softmax warps have read the previous tile's O out of TMEM
-        if (jl == 0 && seg > 0) mbar_wait(&bar->o_free, (seg - 1) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t p_desc = p_desc0 + static_cast<uint64_t>(((it & 1) * P_BYTES) >> 4);
-          const uint64_t v_desc = v_desc0 + static_cast<uint64_t>((st * KV_BYTES) >> 4);
-#pragma unroll
-          for (int k = 0; k < TK / 16; ++k) {
-            umma_f16(tmem_base + TM_O, p_desc + 2 * k, v_desc + static_cast<uint64_t>((k * 16 * 128) >> 4), idesc_o,
-                     (jl > 0 || k != 0) ? 1u : 0u);
-          }
-          umma_commit(&bar->o_full[it & 1]);
-          umma_commit(&bar->kv_empty[st]);
-        }
-        __syncwarp();
-        if (jl + 2 < len) issue_qk(it + 2, jl + 3 == len);      // S buffer it % 2 is free again
-      }
-      g += len;
-    }
-    if (PROBE && p.dbg && lane == 0) p.dbg[8LL * blockIdx.x + 6] = d_wp;
   } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;                 // query row in the tile == TMEM lane
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    const uint32_t t_o = t_lane + TM_O;
+    const int wg = warp >> 2;
+    const int rl0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // tile rows rl0 and rl0 + 8
+    const int cq = 2 * (lane & 3);                              // column of fragment pair j: 8 j + cq
+    const bool signal = (threadIdx.x & 127) == 0;               // one arrival per warpgroup
     const float sl2 = p.scale_log2;
-    const int sw = r & 7;
+    const uint64_t q_desc = wgmma_desc_sw128(smem_u32(sQ)) + static_cast<uint64_t>((wg * 64 * 128) >> 4);
+    const uint64_t k_desc0 = wgmma_desc_sw128(smem_u32(sK));
+    const uint64_t v_desc0 = wgmma_desc_sw128(smem_u32(sV));
     int it = 0, seg = 0;
-    long long d_ws = 0, d_ld = 0, d_wo = 0, d_exp = 0, d_t0 = PROBE && p.dbg ? clock64() : 0;
     for (int g = g_begin; g < g_end; ++seg) {
       const int tile = g / n_steps;
       const int a = g - tile * n_steps;
       const int e = min(g_end, (tile + 1) * n_steps) - tile * n_steps;
       const int qt = tile % p.q_tiles, bh = tile / p.q_tiles;
       const int head = bh % p.heads, b = bh / p.heads;
-      float m_ref = -INFINITY, l_run = 0.f;      // m_ref: the (possibly stale) softmax reference point
+      float m_ref[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // per row: softmax reference point, sum
+      float o[DH / 2];
+#pragma unroll
+      for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+      mbar_wait(&bar->q_full, seg & 1);
 
       for (int j = a; j < e; ++j, ++it) {
-        const int bsel = it & 1;
+        const int st = it % KV_STAGES;
         const int valid = min(TK, p.skv - j * TK);
-        long long c0s = 0, c1s = 0, c2s = 0, c3s = 0;
-        if (PROBE && p.dbg) c0s = clock64();
-        mbar_wait(&bar->s_full[bsel], (it >> 1) & 1);
-        if (PROBE && p.dbg) c1s = clock64();
-        tc_fence_after();
-        uint32_t s[TK];
-        __syncwarp();
-        tmem_ld32(t_lane + TM_S + bsel * TK, s);
-        tmem_ld32(t_lane + TM_S + bsel * TK + 32, s + 32);
-        tmem_ld_wait();
-        // independent max chains (a single chain would expose dependent FMNMX latencies)
-        float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-        if (valid == TK) {
+        mbar_wait(&bar->kv_full[st], (it / KV_STAGES) & 1);
+        float s[TK / 2];
 #pragma unroll
-          for (int i = 0; i < TK; ++i) mx[i & 3] = fmaxf(mx[i & 3], __uint_as_float(s[i]));
-        } else {
+        for (int i = 0; i < TK / 2; ++i) s[i] = 0.f;
+        wgmma_fence();
+        const uint64_t k_desc = k_desc0 + static_cast<uint64_t>((st * KV_BYTES) >> 4);
 #pragma unroll
-          for (int i = 0; i < TK; ++i)
-            if (i < valid) mx[i & 3] = fmaxf(mx[i & 3], __uint_as_float(s[i]));
+        for (int k = 0; k < DH / 16; ++k) wgmma_ss_n64(s, q_desc + 2 * k, k_desc + 2 * k);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_reg_fence(s, TK / 2);
+        if (j == e - 1 && signal) mbar_arrive(&bar->q_empty);     // Q may be replaced
+        if (valid < TK) {
+#pragma unroll
+          for (int i = 0; i < TK / 2; ++i)
+            if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
         }
-        const float m_tile = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-        if (j == a) {
-          m_ref = m_tile;
-        } else {
-          // raise the reference only when this row's max outgrew it by 2^RESCALE_LOG2; warp-uniform
-          // decision because tcgen05.ld/st are warp-collective
-          const bool grow = (m_tile - m_ref) * sl2 > RESCALE_LOG2;
-          if (__any_sync(0xffffffffu, grow)) {
-            const float m_new = grow ? m_tile : m_ref;
-            const float alpha = ex2_approx((m_ref - m_new) * sl2);
-            // PV of the previous step must have retired before O is rescaled
-            mbar_wait(&bar->o_full[(it - 1) & 1], ((it - 1) >> 1) & 1);
-            tc_fence_after();
 #pragma unroll
-            for (int c0 = 0; c0 < DH; c0 += 16) {
-              uint32_t o[16];
-              tmem_ld16(t_o + c0, o);
-              tmem_ld_wait();
+        for (int h = 0; h < 2; ++h) {
+          float mx = -INFINITY;
 #pragma unroll
-              for (int i = 0; i < 16; i += 2) {
-                float y0, y1;
-                fmul2(y0, y1, __uint_as_float(o[i]), __uint_as_float(o[i + 1]), alpha, alpha);
-                o[i] = __float_as_uint(y0); o[i + 1] = __float_as_uint(y1);
-              }
-              tmem_st16(t_o + c0, o);
+          for (int jj = 0; jj < TK / 8; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]));
+          mx = quad_max(mx);
+          if (j == a) {
+            m_ref[h] = mx;
+          } else if ((mx - m_ref[h]) * sl2 > RESCALE_LOG2) {
+            const float alpha = ex2_approx((m_ref[h] - mx) * sl2);
+#pragma unroll
+            for (int jj = 0; jj < DH / 8; ++jj) {
+              o[4 * jj + 2 * h] *= alpha;
+              o[4 * jj + 2 * h + 1] *= alpha;
             }
-            tmem_st_wait();
-            l_run *= alpha;
-            m_ref = m_new;
+            l_run[h] *= alpha;
+            m_ref[h] = mx;
           }
         }
-        // the PV that read this P buffer two steps ago must have retired
-        if (PROBE && p.dbg) c2s = clock64();
-        if (it >= 2) mbar_wait(&bar->o_full[bsel], ((it - 2) >> 1) & 1);
-        if (PROBE && p.dbg) c3s = clock64();
-        uint8_t* p_row = sP + bsel * P_BYTES + r * 128;
-        const float nmb = -m_ref * sl2;
-        float ls[8];
+        // P = exp2(s * scale - m_ref * scale) in 16 bit, laid out as the A fragments of the PV MMAs
+        const float nmb[2] = {-m_ref[0] * sl2, -m_ref[1] * sl2};
+        uint32_t pa[TK / 16][4];
+        float ls[2] = {0.f, 0.f};
 #pragma unroll
-        for (int i = 0; i < 8; ++i) ls[i] = 0.f;
-        if (valid == TK) {
-          // full step: packed FFMA2 / FADD2, no masking
-#pragma unroll
-          for (int c0 = 0; c0 < TK; c0 += 8) {
-            float ex[8];
-#pragma unroll
-            for (int i = 0; i < 8; i += 2) {
-              float x0, x1;
-              ffma2(x0, x1, __uint_as_float(s[c0 + i]), __uint_as_float(s[c0 + i + 1]), sl2, sl2, nmb, nmb);
-              ex[i] = ex2_approx(x0);
-              ex[i + 1] = ex2_approx(x1);
-              fadd2(ls[i], ls[i + 1], ls[i], ls[i + 1], ex[i], ex[i + 1]);
-            }
-            uint4 t;
-            t.x = pack2(ex[0], ex[1]); t.y = pack2(ex[2], ex[3]); t.z = pack2(ex[4], ex[5]); t.w = pack2(ex[6], ex[7]);
-            *reinterpret_cast<uint4*>(p_row + (((c0 >> 3) ^ sw) << 4)) = t;      // 128-byte swizzle
-          }
-        } else {
-#pragma unroll
-          for (int c0 = 0; c0 < TK; c0 += 8) {
-            float ex[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float x = ex2_approx(fmaf(__uint_as_float(s[c0 + i]), sl2, nmb));
-              ex[i] = c0 + i < valid ? x : 0.f;
-              ls[i] += ex[i];
-            }
-            uint4 t;
-            t.x = pack2(ex[0], ex[1]); t.y = pack2(ex[2], ex[3]); t.z = pack2(ex[4], ex[5]); t.w = pack2(ex[6], ex[7]);
-            *reinterpret_cast<uint4*>(p_row + (((c0 >> 3) ^ sw) << 4)) = t;
-          }
+        for (int i = 0; i < TK / 2; i += 2) {
+          const int h = (i >> 1) & 1;
+          const float x0 = ex2_approx(fmaf(s[i], sl2, nmb[h]));
+          const float x1 = ex2_approx(fmaf(s[i + 1], sl2, nmb[h]));
+          ls[h] += x0 + x1;
+          pa[i >> 3][(i >> 1) & 3] = pack2(x0, x1);
         }
-        l_run += ((ls[0] + ls[1]) + (ls[2] + ls[3])) + ((ls[4] + ls[5]) + (ls[6] + ls[7]));
-        tc_fence_before();
-        fence_proxy_async_smem();
-        mbar_arrive(&bar->p_full[bsel]);
-        if (PROBE && p.dbg) { d_ws += c1s - c0s; d_ld += c2s - c1s; d_wo += c3s - c2s; d_exp += clock64() - c3s; }
+        l_run[0] += ls[0];
+        l_run[1] += ls[1];
+        wgmma_fence();
+        const uint64_t v_desc = v_desc0 + static_cast<uint64_t>((st * KV_BYTES) >> 4);
+#pragma unroll
+        for (int kk = 0; kk < TK / 16; ++kk) wgmma_rs_n64_tb(o, pa[kk], v_desc + static_cast<uint64_t>((kk * 16 * 128) >> 4));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_reg_fence(o, DH / 2);
+        if (signal) mbar_arrive(&bar->kv_empty[st]);
       }
-      // ---- end of segment: O (fp32, unnormalised) out of TMEM ----
-      mbar_wait(&bar->o_full[(it - 1) & 1], ((it - 1) >> 1) & 1);
-      tc_fence_after();
-      float o[DH];
-      {
-        uint32_t u[DH];
-        __syncwarp();
-        tmem_ld32(t_o, u);
-        tmem_ld32(t_o + 32, u + 32);
-        tmem_ld_wait();
-#pragma unroll
-        for (int c = 0; c < DH; ++c) o[c] = __uint_as_float(u[c]);
-      }
-      tc_fence_before();
-      mbar_arrive(&bar->o_free);                 // the next tile's first PV may overwrite O
-      const int qi = qt * TQ + r;
-      op_t* o_ptr = reinterpret_cast<op_t*>(p.out) + (static_cast<long long>(b) * p.sq + qi) * p.ldo + head * DH;
+      l_run[0] = quad_sum(l_run[0]);
+      l_run[1] = quad_sum(l_run[1]);
+
       const bool whole = !SK || (a == 0 && e == n_steps);
-      float inv = 1.0f / l_run;
+      float inv[2] = {1.0f / l_run[0], 1.0f / l_run[1]};
       bool store = whole;
       if (!whole) {
         // part of a tile that a CTA boundary cuts: publish (O, m_ref, l), the last part combines
         const int t0 = tile * n_steps;
         const int c_lo = sk_owner(p, t0), c_hi = sk_owner(p, t0 + n_steps - 1);
         const int parts = c_hi - c_lo + 1, part = static_cast<int>(blockIdx.x) - c_lo;
-        // part layout [WS_ROW planes][128 rows]: a warp's 32 rows of one plane are one 128-byte line
-        float* wcol = p.ws + (static_cast<long long>(tile) * p.parts_max + part) * (TQ * WS_ROW) + r;
+        // part layout [WS_ROW planes][128 rows]
+        float* wp = p.ws + (static_cast<long long>(tile) * p.parts_max + part) * (TQ * WS_ROW);
 #pragma unroll
-        for (int c = 0; c < DH; ++c) __stcg(wcol + c * TQ, o[c]);
-        __stcg(wcol + DH * TQ, m_ref);
-        __stcg(wcol + (DH + 1) * TQ, l_run);
+        for (int h = 0; h < 2; ++h) {
+          const int rl = rl0 + 8 * h;
+#pragma unroll
+          for (int jj = 0; jj < DH / 8; ++jj) {
+            __stcg(wp + (8 * jj + cq) * TQ + rl, o[4 * jj + 2 * h]);
+            __stcg(wp + (8 * jj + cq + 1) * TQ + rl, o[4 * jj + 2 * h + 1]);
+          }
+          if ((lane & 3) == 0) {
+            __stcg(wp + DH * TQ + rl, m_ref[h]);
+            __stcg(wp + (DH + 1) * TQ + rl, l_run[h]);
+          }
+        }
         __threadfence();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (threadIdx.x == 64) {
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (threadIdx.x == 0) {
           const unsigned int t = atomicAdd(&p.tickets[tile], 1u);
           const bool last = t == static_cast<unsigned int>(parts) - 1;
           if (last) p.tickets[tile] = 0;           // self-reset for the next launch
           bar->last_flag = last ? 1u : 0u;
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        asm volatile("bar.sync 1, 256;" ::: "memory");
         if (bar->last_flag) {
           __threadfence();
-          const float* base = p.ws + static_cast<long long>(tile) * p.parts_max * (TQ * WS_ROW) + r;
-          float m_all = -INFINITY;
-          for (int i = 0; i < parts; ++i)
-            m_all = fmaxf(m_all, __ldcg(base + static_cast<long long>(i) * TQ * WS_ROW + DH * TQ));
+          const float* base = p.ws + static_cast<long long>(tile) * p.parts_max * (TQ * WS_ROW);
 #pragma unroll
-          for (int c = 0; c < DH; ++c) o[c] = 0.f;    // this CTA's own part is re-read from ws like the others
-          float l_all = 0.f;
-          for (int i = 0; i < parts; ++i) {        // fixed order: deterministic
-            const float* pr = base + static_cast<long long>(i) * TQ * WS_ROW;
-            const float wgt = ex2_approx((__ldcg(pr + DH * TQ) - m_all) * sl2);
-            l_all += __ldcg(pr + (DH + 1) * TQ) * wgt;
+          for (int h = 0; h < 2; ++h) {
+            const int rl = rl0 + 8 * h;
+            float m_all = -INFINITY;
+            for (int i = 0; i < parts; ++i)
+              m_all = fmaxf(m_all, __ldcg(base + static_cast<long long>(i) * TQ * WS_ROW + DH * TQ + rl));
 #pragma unroll
-            for (int c = 0; c < DH; ++c) o[c] += __ldcg(pr + c * TQ) * wgt;
+            for (int jj = 0; jj < DH / 8; ++jj) { o[4 * jj + 2 * h] = 0.f; o[4 * jj + 2 * h + 1] = 0.f; }
+            float l_all = 0.f;
+            for (int i = 0; i < parts; ++i) {        // fixed order: deterministic
+              const float* pr = base + static_cast<long long>(i) * TQ * WS_ROW;
+              const float wgt = ex2_approx((__ldcg(pr + DH * TQ + rl) - m_all) * sl2);
+              l_all += __ldcg(pr + (DH + 1) * TQ + rl) * wgt;
+#pragma unroll
+              for (int jj = 0; jj < DH / 8; ++jj) {
+                o[4 * jj + 2 * h] += __ldcg(pr + (8 * jj + cq) * TQ + rl) * wgt;
+                o[4 * jj + 2 * h + 1] += __ldcg(pr + (8 * jj + cq + 1) * TQ + rl) * wgt;
+              }
+            }
+            inv[h] = 1.0f / l_all;
           }
-          inv = 1.0f / l_all;
           store = true;
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");      // last_flag is reused by the next segment
+        asm volatile("bar.sync 1, 256;" ::: "memory");      // last_flag is reused by the next segment
       }
-      if (store && qi < p.sq) {
+      if (store) {
 #pragma unroll
-        for (int c = 0; c < DH; c += 8) {
-          uint4 t;
-          t.x = pack2(o[c] * inv, o[c + 1] * inv);
-          t.y = pack2(o[c + 2] * inv, o[c + 3] * inv);
-          t.z = pack2(o[c + 4] * inv, o[c + 5] * inv);
-          t.w = pack2(o[c + 6] * inv, o[c + 7] * inv);
-          *reinterpret_cast<uint4*>(o_ptr + c) = t;
+        for (int h = 0; h < 2; ++h) {
+          const int qi = qt * TQ + rl0 + 8 * h;
+          if (qi >= p.sq) continue;
+          op_t* o_ptr = reinterpret_cast<op_t*>(p.out) + (static_cast<long long>(b) * p.sq + qi) * p.ldo + head * DH + cq;
+#pragma unroll
+          for (int jj = 0; jj < DH / 8; ++jj)
+            *reinterpret_cast<uint32_t*>(o_ptr + 8 * jj) = pack2(o[4 * jj + 2 * h] * inv[h], o[4 * jj + 2 * h + 1] * inv[h]);
         }
       }
       g += e - a;
     }
-    if (PROBE && p.dbg && threadIdx.x == 64) {
-      long long* d = p.dbg + 8LL * blockIdx.x;
-      d[0] = clock64() - d_t0; d[1] = d_ws; d[2] = d_ld; d[3] = d_wo; d[4] = d_exp; d[5] = it;
-    }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
@@ -430,20 +306,12 @@ int make_qkv_map(CUtensorMap* m, const void* base, int batch, int s, long long l
 }  // namespace
 
 namespace {
-long long* g_attn_dbg = nullptr;
-}
-/* calibration only: per-CTA clock64 sums of the next attention launches go to `buf` ([ctas][8] int64), NULL = off */
-#ifdef DBIR_DEBUG_PROBES
-extern "C" void dbir_debug_attn_stamps(void* buf) { g_attn_dbg = reinterpret_cast<long long*>(buf); }
-#endif
-
-namespace {
 // Stream-K decomposition: used when whole tiles would leave the last wave of CTA slots (two per SM)
-// mostly empty, e.g. 320 tiles on 296 slots. Returns the grid size; *parts_max = 0 without stream-K.
+// mostly empty, e.g. 320 tiles on 264 slots. Returns the grid size; *parts_max = 0 without stream-K.
 int attn_plan(int batch, int heads, int sq, int skv, int* parts_max) {
   const int q_tiles = (sq + TQ - 1) / TQ, n_steps = (skv + TK - 1) / TK;
   const long long tiles = static_cast<long long>(batch) * heads * q_tiles;
-  const long long slots = 2LL * dbir_sm_count();
+  const long long slots = static_cast<long long>(CTAS_PER_SM) * dbir_sm_count();
   *parts_max = 0;
   static const int sk_mode = [] { const char* e = getenv("DBIR_ATTN_STREAMK"); return e ? atoi(e) : 1; }();
   // (the ticket array holds 16384 tiles; such grids are many waves deep and need no balancing)
@@ -498,7 +366,6 @@ extern "C" int dbir_attention_sk(const void* q, const void* k, const void* v, vo
     parts_max = 0;
   }
   p.parts_max = parts_max;
-  p.dbg = g_attn_dbg;
   if (parts_max > 0) {
     p.tickets = reinterpret_cast<unsigned int*>(ws);
     p.ws = reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + ATTN_TICKET_BYTES);
@@ -510,10 +377,10 @@ extern "C" int dbir_attention_sk(const void* q, const void* k, const void* v, vo
     configured = true;
   }
   if (parts_max > 0)
-    DBIR_CHECK_CUDA(dbir_launch(attn_fwd_kernel<true>, dim3(ctas), dim3(192), ATTN_SMEM,
+    DBIR_CHECK_CUDA(dbir_launch(attn_fwd_kernel<true>, dim3(ctas), dim3(ATTN_THREADS), ATTN_SMEM,
                                 reinterpret_cast<cudaStream_t>(stream), mq, mk, mv, p));
   else
-    DBIR_CHECK_CUDA(dbir_launch(attn_fwd_kernel<false>, dim3(ctas), dim3(192), ATTN_SMEM,
+    DBIR_CHECK_CUDA(dbir_launch(attn_fwd_kernel<false>, dim3(ctas), dim3(ATTN_THREADS), ATTN_SMEM,
                                 reinterpret_cast<cudaStream_t>(stream), mq, mk, mv, p));
   return 0;
 }

@@ -1,9 +1,8 @@
-// diffbir_b200 — shared device/host helpers for the sm_100a kernels.
+// diffbir_b200 — shared device/host helpers for the sm_90a (Hopper) kernels.
 //
-// Everything here is hand-written PTX for Blackwell (mbarrier, TMA, tcgen05/TMEM);
-// no CUTLASS/CuTe types. Encodings follow the PTX ISA; the bit layouts of the
-// UMMA shared-memory descriptor and instruction descriptor are restated in
-// DESIGN.md §"tcgen05 descriptors".
+// Everything here is hand-written PTX (mbarrier, TMA, clusters, wgmma); no CUTLASS/CuTe
+// types. Encodings follow the PTX ISA (the wgmma shared-memory descriptor: "Matrix Descriptor
+// Format" of the asynchronous warpgroup-level matrix instructions); see wgmma_desc_sw128 below.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -14,16 +13,15 @@
 
 // ---------------------------------------------------------------------------
 // 16-bit tensor-core operand format. fp16 (11-bit significand) by default:
-// same tcgen05 kind::f16 throughput as bf16, 8x smaller operand rounding error,
+// same wgmma throughput as bf16, 8x smaller operand rounding error,
 // which is what lets the 50-step trajectory stay >= 50 dB from the fp32
 // reference. Build with -DDBIR_OPERAND_BF16 for bf16 operands.
-// Accumulation is always fp32 (TMEM); residual streams are fp32 in HBM.
+// Accumulation is always fp32 (registers); residual streams are fp32 in HBM.
 // ---------------------------------------------------------------------------
 #ifdef DBIR_OPERAND_BF16
 typedef __nv_bfloat16 op_t;
 typedef __nv_bfloat162 op2_t;
 #define DBIR_OPERAND_KIND 0
-#define DBIR_UMMA_FMT 1u
 __device__ __forceinline__ op_t f2op(float x) { return __float2bfloat16_rn(x); }
 __device__ __forceinline__ float op2f(op_t x) { return __bfloat162float(x); }
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
@@ -38,7 +36,6 @@ __device__ __forceinline__ float2 unpack2(uint32_t u) {
 typedef __half op_t;
 typedef __half2 op2_t;
 #define DBIR_OPERAND_KIND 1
-#define DBIR_UMMA_FMT 0u
 __device__ __forceinline__ op_t f2op(float x) { return __float2half_rn(x); }
 __device__ __forceinline__ float op2f(op_t x) { return __half2float(x); }
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
@@ -84,11 +81,10 @@ extern "C" int dbir_sm_count(void);
 // ---------------------------------------------------------------------------
 // Programmatic dependent launch (PDL): every kernel is launched with the programmatic-stream-serialization
 // attribute (on by default, DBIR_PDL=0 turns it off); each one calls pdl_trigger() at entry (lets the NEXT
-// kernel's CTAs be scheduled and run their prologue: barrier init, TMEM alloc, descriptor prefetch) and
+// kernel's CTAs be scheduled and run their prologue: barrier init, descriptor prefetch) and
 // pdl_wait() before touching memory written by its predecessors (griddepcontrol.wait returns when all
-// prerequisite grids completed and flushed). Measured on B200 inside the captured forward graph (round 2,
-// profiles/r02_forward_ab_4.jsonl): 5.80 ms with it, 5.76 ms without -- the ~200 KB shared-memory GEMM CTAs
-// cannot co-reside with their successor's CTAs, so there is little to overlap; it is harmless and stays on.
+// prerequisite grids completed and flushed). The ~200 KB shared-memory GEMM CTAs cannot co-reside with
+// their successor's CTAs, so there is little to overlap there; the smaller kernels' prologues do overlap.
 // ---------------------------------------------------------------------------
 extern "C" int dbir_pdl_enabled(void);
 template <typename... KArgs, typename... Args>
@@ -133,7 +129,7 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 
 // One lane of a fully converged warp (deterministic for a given mask). Single-thread work
-// (TMA, tcgen05.mma, tcgen05.commit) sits in `if (elect_one())` inside warp-uniform loops: the
+// (TMA issue, barrier arrivals) sits in `if (elect_one())` inside warp-uniform loops: the
 // compiler then keeps addresses / descriptors in uniform registers instead of wrapping every
 // such instruction in a per-lane serialisation loop, which a plain `if (lane == 0)` region costs.
 __device__ __forceinline__ bool elect_one() {
@@ -172,28 +168,19 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a pipeline bug traps (-> launch error) instead of hanging the GPU.
+// Bounded wait: a pipeline bug traps (-> launch error) instead of hanging the GPU. No printf here: a
+// function call in a kernel that issues wgmma makes ptxas serialise every wgmma (C7510).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {  // ~2 s at 2 GHz
-      printf("dbir: mbarrier timeout block(%d,%d,%d) thread %d\n", blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();  // ~2 s at 2 GHz
   }
 }
 
-// ---- proxy / tcgen05 fences ------------------------------------------------
+// ---- proxy fence -----------------------------------------------------------
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---- TMA -------------------------------------------------------------------
@@ -226,109 +213,90 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ---- TMEM ------------------------------------------------------------------
-// Whole-warp (.sync.aligned) calls.
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32-bit, 16 / 32 consecutive columns: thread t of the warp reads TMEM lane
-// (warp%4)*32 + t. taddr = (lane << 16) | column.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,"
-      "%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,"
-      "%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-      "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]),
-      "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// ---- UMMA ------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128B swizzle, rows of 128 bytes, 8-row groups
-// 1024 bytes apart (SBO). Works for K-major operands ([rows][64 x 16-bit]) and for
-// MN-major operands ([k rows][64 x 16-bit of the MN dimension]) alike; `lbo_bytes`
-// only matters for MN-major operands wider than 64 elements.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes = 16) {
+// ---- wgmma -----------------------------------------------------------------
+// Shared-memory matrix descriptor, 128B swizzle, rows of 128 bytes, 8-row groups 1024 bytes apart
+// (SBO). Works for K-major operands ([rows][64 x 16-bit]) and for MN-major operands ([k rows][64 x
+// 16-bit of the MN dimension], one swizzle atom wide) alike. Stage buffers are 1024-byte aligned, so
+// the base-offset field stays 0; the start address advances in 16-byte units (+2 per 16-wide k step
+// inside a K-major atom).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((1024u >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;  // descriptor version (Blackwell)
-  d |= 2ull << 61;  // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 16;                        // LBO (unused by swizzled K-major)
+  d |= static_cast<uint64_t>((1024u >> 4) & 0x3FFF) << 32;    // SBO
+  d |= 1ull << 62;                                            // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16, fp32 accumulate, M=128.
-__host__ __device__ constexpr uint32_t umma_idesc(uint32_t n, uint32_t a_mn_major,
-                                                  uint32_t b_mn_major, uint32_t m = 128u) {
-  return (1u << 4) | (DBIR_UMMA_FMT << 7) | (DBIR_UMMA_FMT << 10) | (a_mn_major << 15) |
-         (b_mn_major << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrives on the mbarrier once all previously issued MMAs of this thread completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::
-                   "r"(smem_u32(bar))
-               : "memory");
+// Keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs.
+__device__ __forceinline__ void wgmma_reg_fence(float* d, int n) {
+  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- CTA pair (cta_group::2): two CTAs of a cluster on the two SMs of a TPC run one M=256 MMA;
-// each CTA holds its own 128 accumulator rows in its TMEM and stages its 128 rows of A plus HALF
-// of the B tile, so the B operand crosses the L2 fabric once per pair instead of once per CTA.
+#ifdef DBIR_OPERAND_BF16
+#define DBIR_WGMMA_AB "bf16.bf16"
+#else
+#define DBIR_WGMMA_AB "f16.f16"
+#endif
+// D[64 x N] += A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory, fp32 accumulator in
+// registers: d[4 j + {0,1}] = (row w*16 + lane/4, col 8 j + 2 (lane%4) + {0,1}), d[4 j + {2,3}] = row + 8
+// (w = warp of the warpgroup).
+__device__ __forceinline__ void wgmma_ss_n32(float* d, uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32." DBIR_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_ss_n64(float* d, uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." DBIR_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_ss_n128(float* d, uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." DBIR_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_ss_n160(float* d, uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n160k16.f32." DBIR_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, %80, %81, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+      : "l"(da), "l"(db));
+}
+__device__ __forceinline__ void wgmma_ss_n256(float* d, uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32." DBIR_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db));
+}
+// A (P, 64 x 16) from registers in accumulator-fragment order, B MN-major (transposed) in shared memory
+__device__ __forceinline__ void wgmma_rs_n64_tb(float* d, const uint32_t* a, uint64_t db) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." DBIR_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+
+// ---- clusters ----------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -343,72 +311,35 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
   return r;
 }
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+// arrive on an mbarrier of any CTA of the cluster (shared::cluster address)
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// TMA loads whose completion is signalled on a barrier of EITHER CTA of the pair (`bar_cluster` is
-// a shared::cluster address, normally the leader's barrier)
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* m, uint32_t bar_cluster,
-                                                 int c0, int c1) {
+// TMA load written to the same shared-memory offset of every CTA in `mask`; each destination CTA's
+// mbarrier at `bar`'s offset receives the bytes it got
+__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                               uint16_t mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, "
-      "{%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const CUtensorMap* m, uint32_t bar_cluster,
-                                                 int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, "
-      "{%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrives on the barrier at this shared-memory offset in BOTH CTAs of the pair.
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "{\n.reg .b16 m;\nmov.b16 m, 3;\n"
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], m;\n}" ::
-          "r"(smem_u32(bar))
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, "
+      "{%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
 
 // ---- misc math -------------------------------------------------------------
-// Packed fp32 pair arithmetic (FFMA2 / FADD2 / FMUL2 on sm_100): one issue slot for two lanes of work.
+// fp32 pair arithmetic, round-to-nearest and never contracted (same bits as two scalar ops).
 __device__ __forceinline__ void ffma2(float& d0, float& d1, float a0, float a1, float b0, float b1,
                                       float c0, float c1) {
-  asm("{ .reg .b64 ra, rb, rc, rd;\n mov.b64 ra, {%2,%3};\n mov.b64 rb, {%4,%5};\n mov.b64 rc, {%6,%7};\n"
-      " fma.rn.f32x2 rd, ra, rb, rc;\n mov.b64 {%0,%1}, rd; }"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1), "f"(c0), "f"(c1));
+  d0 = __fmaf_rn(a0, b0, c0);
+  d1 = __fmaf_rn(a1, b1, c1);
 }
 __device__ __forceinline__ void fadd2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-  asm("{ .reg .b64 ra, rb, rd;\n mov.b64 ra, {%2,%3};\n mov.b64 rb, {%4,%5};\n"
-      " add.rn.f32x2 rd, ra, rb;\n mov.b64 {%0,%1}, rd; }"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = __fadd_rn(a0, b0);
+  d1 = __fadd_rn(a1, b1);
 }
 __device__ __forceinline__ void fmul2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-  asm("{ .reg .b64 ra, rb, rd;\n mov.b64 ra, {%2,%3};\n mov.b64 rb, {%4,%5};\n"
-      " mul.rn.f32x2 rd, ra, rb;\n mov.b64 {%0,%1}, rd; }"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
+  d0 = __fmul_rn(a0, b0);
+  d1 = __fmul_rn(a1, b1);
 }
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -437,8 +368,7 @@ __device__ __forceinline__ float gelu_erf_f(float x) {
   const float phi = x >= 0.f ? 1.0f - half_erfc : half_erfc;
   return x * phi;
 }
-// Two GELUs per call on packed fp32 pairs (FFMA2 / FMUL2): same A-S 7.1.26 polynomial as gelu_erf_f, half the
-// FMA-pipe issue slots -- the GEGLU epilogue (K = C: the mainloop is only 5-20 k-blocks long) is bound by them.
+// Two GELUs per call on fp32 pairs: the A-S 7.1.26 polynomial of gelu_erf_f, written pairwise.
 __device__ __forceinline__ void gelu_erf_f2(float x0, float x1, float& y0, float& y1) {
   float z0 = fabsf(x0), z1 = fabsf(x1);
   fmul2(z0, z1, z0, z1, 0.70710678118654752f, 0.70710678118654752f);

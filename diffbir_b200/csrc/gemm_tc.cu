@@ -1,6 +1,6 @@
-// tcgen05 / TMEM / TMA GEMM with an implicit-GEMM 3x3 convolution mode.
+// wgmma / TMA GEMM with an implicit-GEMM 3x3 convolution mode (sm_90a).
 //
-//   D[M, N] = A[M, K] * B[N, K]^T   (16-bit operands, fp32 accumulate in TMEM)
+//   D[M, N] = A[M, K] * B[N, K]^T   (16-bit operands, fp32 accumulate in registers)
 //
 // A is either a plain row-major [M, K] matrix (Linear layers, 1x1 convs on NHWC
 // activations) or an NHWC activation tensor read through a 4-D TMA box, one box per
@@ -8,15 +8,16 @@
 // (replaces nn.Conv2d 3x3/pad 1 at reference unet.py:149-153,173-180, vae.py:77-86,
 // swinir.py:472,797-811). B is the packed weight [N, K] (K = taps*C, tap-major).
 //
-// One CTA computes a 128 x BN tile: warp 0 = TMA producer, warp 1 = MMA issuer,
-// warp 2 = TMEM allocator + epilogue, warps 3..5 = epilogue (thread == accumulator row).
+// One CTA computes a 128 x BN tile: warps 0-7 are two consumer warpgroups (tile rows 0-63 / 64-127,
+// wgmma with both operands in shared memory, accumulators in registers), warp 8 is the TMA producer.
+// After the mainloop the accumulators go to the freed stage memory as swizzled 32 x 32 fp32 blocks and
+// the same eight warps run the epilogue on them (thread == accumulator row).
 //
-// Epilogue (per warp, 32 rows x 32 columns at a time): tcgen05.ld -> bias / per-image row
+// Epilogue (per warp, 32 rows x 32 columns at a time): accumulator block -> bias / per-image row
 // vector (time embedding) / GELU / LeakyReLU / SiLU / GEGLU gating / alpha -> + fp32 residual
 // tile (TMA-loaded, double buffered) -> swizzled shared-memory tile -> TMA bulk store
-// (double buffered). Threads never touch global memory for the output: with one epilogue warp
-// per scheduler every extra instruction is exposed latency, and the TMA unit also clips
-// overhanging rows / columns (M, N tails, conv tiles that overhang the image).
+// (from the accumulator block itself). Threads never touch global memory for the output, and the TMA
+// unit clips overhanging rows / columns (M, N tails, conv tiles that overhang the image).
 //   out = residual + alpha * act(acc + bias + rowvec),  fp32 or 16-bit, any row stride.
 #include "common.cuh"
 #include "../../include/diffbir_b200.h"
@@ -105,14 +106,15 @@ __device__ __forceinline__ void bulk_wait_read() {
 struct EpiCtx {
   const CUtensorMap* tm_out;
   const CUtensorMap* tm_res;
-  uint32_t epi_base;       // shared address of this warp's 4 staging tiles: out[0], out[1], res[0], res[1]
+  uint32_t cur;            // shared address of the chunk being finished: its accumulator block, reused as the
+                           // output staging tile
+  uint32_t res_base;       // this warp's two residual staging tiles
   uint32_t res_bar;        // shared address of this warp's two residual-load mbarriers
   int row0;                // plain mode: first global row of this warp
   int x, y, n;             // conv mode: origin of this warp's sub-box
   long long stats_base;    // element offset of this warp's (image, slot) row in the stats buffer, < 0: none
   int grp_off;             // grouped launch: row offset of this CTA's problem in the stacked bias
-  __device__ __forceinline__ uint32_t out_buf(int b) const { return epi_base + b * EPI_TILE_BYTES; }
-  __device__ __forceinline__ uint32_t res_buf(int b) const { return epi_base + (2 + b) * EPI_TILE_BYTES; }
+  __device__ __forceinline__ uint32_t res_buf(int b) const { return res_base + b * EPI_TILE_BYTES; }
   __device__ __forceinline__ uint32_t bar(int b) const { return res_bar + b * 8; }
 };
 
@@ -125,7 +127,7 @@ __device__ __forceinline__ void mbar_wait_s(uint32_t bar, uint32_t parity) {
         : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     if (ok) return;
     if (t0 == 0) t0 = clock64();
-    else if (clock64() - t0 > 4000000000LL) { printf("dbir: residual mbarrier timeout\n"); __trap(); }
+    else if (clock64() - t0 > 4000000000LL) __trap();     // no printf: see mbar_wait
   }
 }
 
@@ -222,17 +224,15 @@ __device__ __forceinline__ void finish_chunk(const GemmParams& p, EpiCtx& e, flo
     __syncwarp();                                   // every lane has read the residual tile
     if (next_gc0 >= 0) epi_issue_residual(p, e, lane, chunk_idx + 2, next_gc0);
   }
-  // the store that used this staging buffer two chunks ago must have finished reading it
-  if (lane == 0 && chunk_idx >= 2) bulk_wait_read<1>();
-  __syncwarp();
+  __syncwarp();                                   // every lane has read the chunk out of its block
   if (p.out_kind == 0) {
-    const uint32_t orow = e.out_buf(b) + lane * 128;          // 128-byte rows, SWIZZLE_128B
+    const uint32_t orow = e.cur + lane * 128;          // 128-byte rows, SWIZZLE_128B
 #pragma unroll
     for (int j = 0; j < 8; ++j)
       sts_v4(orow + ((j ^ sw) << 4), __float_as_uint(v[4 * j]), __float_as_uint(v[4 * j + 1]),
              __float_as_uint(v[4 * j + 2]), __float_as_uint(v[4 * j + 3]));
   } else {
-    const uint32_t orow = e.out_buf(b) + lane * 64;           // 64-byte rows, SWIZZLE_64B
+    const uint32_t orow = e.cur + lane * 64;           // 64-byte rows, SWIZZLE_64B
     const int sw2 = (lane >> 1) & 3;
 #pragma unroll
     for (int j = 0; j < 4; ++j)
@@ -250,50 +250,76 @@ __device__ __forceinline__ void finish_chunk(const GemmParams& p, EpiCtx& e, flo
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       float x;
-      asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(e.out_buf(b) + i * 128 + (((chunk ^ (i & 7))) << 4) + col_off) : "memory");
+      asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(e.cur + i * 128 + (((chunk ^ (i & 7))) << 4) + col_off) : "memory");
       if ((valid >> i) & 1u) { sa += x; sb += x * x; }
     }
     if (lane < ncols)
       *reinterpret_cast<float2*>(p.stats + (e.stats_base + gc0 + lane) * 2) = make_float2(sa, sb);
   }
   if (lane == 0) {
-    if (p.mode == 0) tma_store_2d(e.tm_out, e.out_buf(b), gc0, e.row0);
-    else tma_store_4d(e.tm_out, e.out_buf(b), gc0, e.x, e.y, e.n);
+    if (p.mode == 0) tma_store_2d(e.tm_out, e.cur, gc0, e.row0);
+    else tma_store_4d(e.tm_out, e.cur, gc0, e.x, e.y, e.n);
     bulk_commit();
   }
 }
 
-// EW = number of epilogue warps: 4 (two CTAs per SM, epilogue of one overlaps the mainloop of the
-// other) or 8 (grids that leave <= 1 CTA per SM: two warps per TMEM lane quarter take alternate
-// 32-column chunks, halving the exposed epilogue latency).
-// PAIR: the two CTAs of a (2,1,1) cluster (adjacent M tiles, same N tile) run M=256 MMAs issued by
-// the even CTA (cta_group::2); each CTA stages its own A rows and half of the B tile.
-// KSUB: 64-wide k-blocks per pipeline stage. The producer / MMA-issue loops cost ~350-500 cycles per
-// iteration in barrier, TMA-issue and commit latency (measured), more than the MMAs of one k-block
-// take for BN < 256; two k-blocks per stage amortise that.
-template <int BN, int STAGES, int EW, bool PAIR, int KSUB>
-__global__ void __launch_bounds__(64 + 32 * EW, EW == 4 ? 2 : 1)
+constexpr int EW = 8;                        // epilogue warps == the two consumer warpgroups
+constexpr int PRODUCER_WARP = EW;
+constexpr int GEMM_THREADS = 32 * EW + 32;
+constexpr int CSTEP = 64;                    // two warps per 32-row quarter take alternate 32-column chunks
+
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db) {
+  if constexpr (BN == 32) wgmma_ss_n32(d, da, db);
+  else if constexpr (BN == 64) wgmma_ss_n64(d, da, db);
+  else if constexpr (BN == 128) wgmma_ss_n128(d, da, db);
+  else if constexpr (BN == 160) wgmma_ss_n160(d, da, db);
+  else wgmma_ss_n256(d, da, db);
+}
+
+// Accumulator block (32-column chunk c, 32-row quarter q): [32 rows][32 fp32], 128-byte rows with the
+// 16-byte units XOR-swizzled by (row & 7) -- the layout of the SWIZZLE_128B output / residual boxes.
+__device__ __forceinline__ uint32_t acc_block(uint32_t base, int c, int q) {
+  return base + static_cast<uint32_t>(c * 4 + q) * EPI_TILE_BYTES;
+}
+// thread == row `lane` of the block: its 32 values
+__device__ __forceinline__ void acc_ld32(uint32_t blk, int lane, float* v) {
+  const uint32_t row = blk + lane * 128;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 t = lds_v4(row + ((j ^ (lane & 7)) << 4));
+    v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w;
+  }
+}
+
+template <int BN, int STAGES>
+struct GemmSmem {
+  static constexpr int B_STAGE_BYTES = BN * BK * 2;
+  static constexpr int PIPE = STAGES * (A_SUB_BYTES + B_STAGE_BYTES);
+  static constexpr int EPI = BN * BM * 4 + EW * 2 * EPI_TILE_BYTES;     // accumulator blocks + residual tiles
+  static constexpr int DATA = PIPE > EPI ? PIPE : EPI;
+  static constexpr int TOTAL = DATA + 1024 + 512;                        // + alignment slack, barriers
+};
+
+// PAIR: the two CTAs of a (2,1,1) cluster (adjacent M tiles, same N tile) each load half of the B tile
+// and multicast it to both, so B crosses the L2 fabric once per pair; a stage is refilled only after
+// the consumers of both CTAs released it.
+template <int BN, int STAGES, bool PAIR>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                const __grid_constant__ CUtensorMap tma_out, const __grid_constant__ CUtensorMap tma_res,
                const GemmParams p) {
-  constexpr int B_ROWS = PAIR ? BN / 2 : BN;          // B rows staged by this CTA
-  constexpr int B_SUB_BYTES = B_ROWS * BK * 2;        // one k-block of B
-  constexpr int A_STAGE_BYTES = KSUB * A_SUB_BYTES;
-  constexpr int B_STAGE_BYTES = KSUB * B_SUB_BYTES;
-  constexpr uint32_t TMEM_COLS = BN <= 32 ? 32 : BN <= 64 ? 64 : BN <= 128 ? 128 : 256;
-  static_assert(STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) >= EW * 4 * EPI_TILE_BYTES, "epilogue staging must fit in the pipeline stages");
-  constexpr int CSTEP = 32 * (EW / 4);        // column stride between the chunks of one warp
+  using L = GemmSmem<BN, STAGES>;
+  constexpr int B_ROWS = PAIR ? BN / 2 : BN;          // B rows loaded by this CTA
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * A_STAGE_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_STAGE_BYTES);
+  uint8_t* sB = smem + STAGES * A_SUB_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + L::DATA);
   uint64_t* empty = full + STAGES;
-  uint64_t* tmem_full = empty + STAGES;
-  uint64_t* res_bars = tmem_full + 1;                 // [EW warps][2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bars + 2 * EW);
-  uint32_t* split_flag = tmem_slot + 1;
+  uint64_t* res_bars = empty + STAGES;                // [EW warps][2]
+  uint32_t* split_flag = reinterpret_cast<uint32_t*>(res_bars + 2 * EW);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -319,36 +345,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   int grp_off = 0;
   if (p.group_span > 0) grp_off = ((p.mode == 1 ? n0 : m_tile) / p.group_span) * p.N;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
     tma_prefetch_desc(&tma_out);
     if (p.has_residual) tma_prefetch_desc(&tma_res);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], PAIR ? 4 : 2); }
     for (int i = 0; i < 2 * EW; ++i) mbar_init(&res_bars[i], 1);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if constexpr (PAIR) tmem_alloc_pair(tmem_slot, TMEM_COLS);
-    else tmem_alloc(tmem_slot, TMEM_COLS);
-  }
-  tc_fence_before();
-  // PAIR: the peer's barriers and TMEM must be live before any remote complete_tx / MMA write
+  // PAIR: the peer's barriers must be live before any multicast complete_tx or remote arrive
   if constexpr (PAIR) cluster_sync_all();
   else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_trigger();        // the next kernel may start its prologue
   pdl_wait();           // A operand / residual come from predecessor kernels
   if (p.dbg) t_setup = clock64();
 
-  const int n_stage_iters = (kb1 - kb0 + KSUB - 1) / KSUB;
-  if (warp == 0) {
+  const int n_iters = kb1 - kb0;
+  if (warp == PRODUCER_WARP) {
     // ---------------- TMA producer: warp-uniform loop, one elected lane issues -------------
-    const uint32_t fbar0 = PAIR ? mapa_u32(smem_u32(&full[0]), 0) : smem_u32(&full[0]);
     const int b_row = grp_off + n_tile * BN + static_cast<int>(cta_rank) * B_ROWS;
     // conv mode: (channel block, tap column, tap row) of the next k-block, advanced incrementally
     // (integer divisions in this loop cost more than the TMA issue itself)
@@ -361,94 +376,29 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     }
     int s = 0;
     uint32_t ph = 0;
-    for (int it = 0; it < n_stage_iters; ++it) {
-      // coordinates of this stage's k-blocks (all lanes, so they stay in uniform registers).
-      // k-blocks past this CTA's range are fetched from out-of-range coordinates: the TMA unit
-      // zero-fills them without memory traffic and the byte count per stage stays constant.
-      int kc[KSUB], ac[KSUB], ax[KSUB], ay[KSUB];
-#pragma unroll
-      for (int j = 0; j < KSUB; ++j) {
-        const int kb = kb0 + it * KSUB + j;
-        const bool live = kb < kb1;
-        kc[j] = live ? kb * BK : p.num_kb * BK;
-        ac[j] = ax[j] = ay[j] = 0;
-        if (p.mode == 1) {
-          // conv: A is addressed by (channel block, tap offset) instead of k
-          ac[j] = live ? cb * BK : p.cblocks * BK;
-          ax[j] = x0 + tx - p.pad;
-          ay[j] = y0 + ty - p.pad;
-          if (++cb == p.cblocks) { cb = 0; if (++tx == p.kw) { tx = 0; ++ty; } }
-        }
-      }
+    for (int it = 0; it < n_iters; ++it) {
+      const int kc = (kb0 + it) * BK;
+      // conv: A is addressed by (channel block, tap offset) instead of k
+      const int ac = cb * BK, ax = x0 + tx - p.pad, ay = y0 + ty - p.pad;
+      if (p.mode == 1 && ++cb == p.cblocks) { cb = 0; if (++tx == p.kw) { tx = 0; ++ty; } }
       mbar_wait(&empty[s], ph ^ 1);
       if (elect_one()) {
-        // PAIR: both CTAs' loads complete on the leader's barrier, which expects the bytes of both
-        if (cta_rank == 0) mbar_expect_tx(&full[s], (PAIR ? 2 : 1) * (A_STAGE_BYTES + B_STAGE_BYTES));
-        const uint32_t fbar = fbar0 + s * 8;
-#pragma unroll
-        for (int j = 0; j < KSUB; ++j) {
-          uint8_t* a_dst = sA + s * A_STAGE_BYTES + j * A_SUB_BYTES;
-          uint8_t* b_dst = sB + s * B_STAGE_BYTES + j * B_SUB_BYTES;
-          if (p.mode == 0) {
-            if constexpr (PAIR) tma_load_2d_pair(a_dst, &tma_a, fbar, kc[j], m_tile * BM);
-            else tma_load_2d(a_dst, &tma_a, &full[s], kc[j], m_tile * BM);
-          } else {
-            if constexpr (PAIR) tma_load_4d_pair(a_dst, &tma_a, fbar, ac[j], ax[j], ay[j], n0);
-            else tma_load_4d(a_dst, &tma_a, &full[s], ac[j], ax[j], ay[j], n0);
-          }
-          if constexpr (PAIR) tma_load_2d_pair(b_dst, &tma_b, fbar, kc[j], b_row);
-          else tma_load_2d(b_dst, &tma_b, &full[s], kc[j], b_row);
-        }
+        mbar_expect_tx(&full[s], A_SUB_BYTES + L::B_STAGE_BYTES);
+        uint8_t* a_dst = sA + s * A_SUB_BYTES;
+        uint8_t* b_dst = sB + s * L::B_STAGE_BYTES;
+        if (p.mode == 0) tma_load_2d(a_dst, &tma_a, &full[s], kc, m_tile * BM);
+        else tma_load_4d(a_dst, &tma_a, &full[s], ac, ax, ay, n0);
+        if constexpr (PAIR) tma_load_2d_mc(b_dst + cta_rank * (B_ROWS * BK * 2), &tma_b, &full[s], kc, b_row, 3);
+        else tma_load_2d(b_dst, &tma_b, &full[s], kc, b_row);
       }
       __syncwarp();
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer (leader CTA of a pair only): warp-uniform loop -------------
-    if (cta_rank == 0) {
-      constexpr uint32_t idesc = umma_idesc(BN, 0, 0, PAIR ? 256u : 128u);
-      const uint64_t a_desc0 = umma_desc_sw128(smem_u32(sA));
-      const uint64_t b_desc0 = umma_desc_sw128(smem_u32(sB));
-      int s = 0;
-      uint32_t ph = 0;
-      for (int it = 0; it < n_stage_iters; ++it) {
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        if (elect_one()) {
-          // descriptors advance in units of 16 bytes (start-address field, low bits)
-          const uint64_t a_desc = a_desc0 + static_cast<uint64_t>((s * A_STAGE_BYTES) >> 4);
-          const uint64_t b_desc = b_desc0 + static_cast<uint64_t>((s * B_STAGE_BYTES) >> 4);
-#pragma unroll
-          for (int j = 0; j < KSUB; ++j) {
-            if (kb0 + it * KSUB + j < kb1) {
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint64_t da = a_desc + static_cast<uint64_t>((j * A_SUB_BYTES) >> 4) + 2 * k;
-                const uint64_t db = b_desc + static_cast<uint64_t>((j * B_SUB_BYTES) >> 4) + 2 * k;
-                const uint32_t acc = (it > 0 || j > 0 || k > 0) ? 1u : 0u;
-                if constexpr (PAIR) umma_f16_pair(tmem_base, da, db, idesc, acc);
-                else umma_f16(tmem_base, da, db, idesc, acc);
-              }
-            }
-          }
-          // frees the smem stage (in both CTAs of a pair) once these MMAs retire
-          if constexpr (PAIR) umma_commit_pair(&empty[s]);
-          else umma_commit(&empty[s]);
-        }
-        __syncwarp();
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-      // accumulator complete
-      if (elect_one()) {
-        if constexpr (PAIR) umma_commit_pair(tmem_full);
-        else umma_commit(tmem_full);
-      }
-    }
   } else {
-    // ---------------- epilogue: warps 2.., TMEM lane quarter = warp % 4 -------------
+    // ---------------- consumers, then epilogue: warps 0..7, row quarter = warp % 4 -------------
     const int q = warp & 3;
-    const int ew = warp - 2;                // epilogue warp index
-    const int c_first = (ew >> 2) * 32;     // first chunk of this warp (EW == 8: warps 6..9 start at column 32)
+    const int ew = warp;                    // epilogue warp index
+    const int c_first = (ew >> 2) * 32;     // warps 4..7 start at column 32
     const int r = q * 32 + lane;            // accumulator row within the tile
     long long out_row = -1;                 // global output row (bias_per_row / rowvec index), -1 = masked
     int vec_idx = 0;
@@ -460,7 +410,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     e.x = e.y = e.n = 0;
     if (p.mode == 0) {
       const long long gr = static_cast<long long>(m_tile) * BM + r;
-      if (gr < p.M) { out_row = gr; vec_idx = static_cast<int>(gr / p.rows_per_vec); }
+      if (gr < p.M) { out_row = gr; vec_idx = static_cast<int>(gr) / p.rows_per_vec; }   // 32-bit: gr < M
     } else {
       const int bx = r % p.bw;
       const int by = (r / p.bw) % p.bh;
@@ -489,7 +439,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       // one 128-byte line per prefetch; lines are spread over every epilogue thread of the grid
       const long long nthr = static_cast<long long>(gridDim.x) * gridDim.y * gridDim.z * (32 * EW);
       const long long me = ((static_cast<long long>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * (32 * EW) +
-                           (threadIdx.x - 64);
+                           threadIdx.x;
       for (long long off = me * 128; off < p.pf_bytes; off += nthr * 128)
         asm volatile("prefetch.global.L2 [%0];" ::"l"(p.pf_ptr + off));
     }
@@ -520,8 +470,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       }
     }
     // GEGLU: value / gate biases of every chunk this warp finishes (lane == column), fetched while the
-    // mainloop runs and broadcast with shuffles (the per-element __ldg pair this replaces sat on the
-    // epilogue's critical path)
+    // mainloop runs and broadcast through shared memory later
     constexpr int MAX_G = (BN / 2) / CSTEP + 1;
     float pa[MAX_G], pg[MAX_G];
     if (p.geglu) {
@@ -533,12 +482,63 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         pg[i] = live ? __ldg(p.bias + grp_off + n_tile * BN + BN / 2 + c) : 0.f;
       }
     }
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
+
+    // ---------------- mainloop: this warpgroup's 64 rows x BN, one 64-wide k-block per stage ----------
+    const int wg = warp >> 2;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    {
+      const uint64_t a_desc0 = wgmma_desc_sw128(smem_u32(sA)) + static_cast<uint64_t>((wg * 64 * 128) >> 4);
+      const uint64_t b_desc0 = wgmma_desc_sw128(smem_u32(sB));
+      const uint32_t peer_empty = PAIR ? mapa_u32(smem_u32(&empty[0]), cta_rank ^ 1u) : 0u;
+      const bool signal = (threadIdx.x & 127) == 0;       // one arrival per warpgroup
+      auto release = [&](int st) {
+        if (signal) {
+          mbar_arrive(&empty[st]);
+          if constexpr (PAIR) mbar_arrive_cluster(peer_empty + st * 8);
+        }
+      };
+      int s = 0, prev = -1;
+      uint32_t ph = 0;
+      for (int it = 0; it < n_iters; ++it) {
+        mbar_wait(&full[s], ph);
+        wgmma_fence();
+        const uint64_t da = a_desc0 + static_cast<uint64_t>((s * A_SUB_BYTES) >> 4);
+        const uint64_t db = b_desc0 + static_cast<uint64_t>((s * L::B_STAGE_BYTES) >> 4);
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) wgmma_tile<BN>(acc, da + 2 * k, db + 2 * k);
+        wgmma_commit();
+        wgmma_wait<1>();                    // the previous stage's MMAs have retired: hand it back
+        if (prev >= 0) release(prev);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc, BN / 2);
+      if (prev >= 0) release(prev);
+    }
     if (p.dbg) t_acc = clock64();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    // all MMAs have retired -> the pipeline stages are free: 4 staging tiles (4 KB) per warp
-    e.epi_base = smem_u32(sA) + ew * (4 * EPI_TILE_BYTES);
+    // every MMA of both warpgroups has retired -> the stage memory is free: accumulators -> blocks
+    asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
+    const uint32_t acc_base = smem_u32(smem);
+    {
+      const int rw = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // first of this thread's two rows
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = rw + 8 * h, rr = row & 31;
+          const uint32_t addr = acc_block(acc_base, col >> 5, row >> 5) + rr * 128 +
+                                ((((col & 31) >> 2) ^ (rr & 7)) << 4) + (col & 3) * 4;
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(acc[4 * j + 2 * h]),
+                       "f"(acc[4 * j + 2 * h + 1]) : "memory");
+        }
+      }
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
+    e.res_base = acc_base + BN * BM * 4 + ew * (2 * EPI_TILE_BYTES);
 
     constexpr int OUT_COLS = BN;            // accumulator columns that produce output (GEGLU: BN/2)
     const bool finalize = p.splits == 1;
@@ -555,24 +555,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       int ci = 0;
 #pragma unroll 1
       for (int c0 = c_first; c0 < BN; c0 += CSTEP) {
-        uint32_t acc[32];
+        float v[32];
+        e.cur = acc_block(acc_base, c0 >> 5, q);
         __syncwarp();
-        tmem_ld32(taddr + c0, acc);
-        tmem_ld_wait();
+        acc_ld32(e.cur, lane, v);
         const int gc0 = col_base + c0;
         if (p.splits > 1) {
           // raw partial -> workspace [tile][split][col][row]: coalesced across the warp's rows
           float* wcol = p.ws + ((static_cast<long long>(tile_lin) * p.splits + blockIdx.z) * BN + c0) * BM + r;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) __stcg(wcol + j * BM, __uint_as_float(acc[j]));
+          for (int j = 0; j < 32; ++j) __stcg(wcol + j * BM, v[j]);
           continue;
         }
         if (gc0 >= p.N) continue;
         const int ncols = min(32, p.N - gc0);
         const int ngc = gc0 + 2 * CSTEP;
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(acc[j]);
         finish_chunk(p, e, v, lane, ci, gc0, ncols, (c0 + 2 * CSTEP < BN && ngc < p.N) ? ngc : -1, out_row, vec_idx, true,
                      have_pre, pre[(c0 - c_first) / CSTEP]);
         ++ci;
@@ -580,7 +577,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       if (p.splits > 1) {
         __threadfence();
         asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
-        if (threadIdx.x == 64) {
+        if (threadIdx.x == 0) {
           const unsigned int t = atomicAdd(&p.tickets[tile_lin], 1u);
           const bool last = (t == static_cast<unsigned int>(p.splits) - 1);
           if (last) p.tickets[tile_lin] = 0;        // self-reset for the next launch
@@ -611,6 +608,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
 #pragma unroll
               for (int j = 0; j < 32; ++j) v[j] += __ldcg(wcol + j * BM);
             }
+            e.cur = acc_block(acc_base, c0 >> 5, q);
             finish_chunk(p, e, v, lane, cj, gc0, ncols, (c0 + 2 * CSTEP < BN && ngc < p.N) ? ngc : -1, out_row, vec_idx, true,
                          have_pre, pre[(c0 - c_first) / CSTEP]);
             ++cj;
@@ -624,8 +622,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       const int n_half = p.N / 2;
       if constexpr (HB % 32 == 0) {
         // Value / gate biases of this warp's chunks go through its (unused: GEGLU has no residual) residual
-        // staging tile and come back as broadcast LDS.128: 16 loads per chunk instead of 64 shuffles, and the
-        // gating math runs on packed fp32 pairs -- the epilogue's FMA-pipe slots bound this kernel (K = C).
+        // staging tile and come back as broadcast LDS.128: 16 loads per chunk instead of 64 shuffles.
         const uint32_t bb = e.res_buf(0);
 #pragma unroll
         for (int i = 0; i < MAX_G; ++i) {
@@ -638,11 +635,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
         for (int i = 0; i < MAX_G; ++i) {
           const int c0 = c_first + i * CSTEP;
           if (c0 >= HB) break;
-          uint32_t av[32], ag[32];
+          float av[32], ag[32];
+          e.cur = acc_block(acc_base, c0 >> 5, q);
           __syncwarp();
-          tmem_ld32(taddr + c0, av);
-          tmem_ld32(taddr + HB + c0, ag);
-          tmem_ld_wait();
+          acc_ld32(e.cur, lane, av);
+          acc_ld32(acc_block(acc_base, (HB + c0) >> 5, q), lane, ag);
           const int gc0 = n_tile * HB + c0;   // output column
           if (gc0 >= n_half) continue;
           const int ncols = min(32, n_half - gc0);
@@ -651,10 +648,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
           for (int jj = 0; jj < 8; ++jj) {
             const float4 ba = lds_v4(bb + i * 256 + jj * 16), bg = lds_v4(bb + i * 256 + 128 + jj * 16);
             float a0, a1, a2, a3, g0, g1, g2, g3, y0, y1, y2, y3;
-            fadd2(a0, a1, __uint_as_float(av[4 * jj]), __uint_as_float(av[4 * jj + 1]), ba.x, ba.y);
-            fadd2(a2, a3, __uint_as_float(av[4 * jj + 2]), __uint_as_float(av[4 * jj + 3]), ba.z, ba.w);
-            fadd2(g0, g1, __uint_as_float(ag[4 * jj]), __uint_as_float(ag[4 * jj + 1]), bg.x, bg.y);
-            fadd2(g2, g3, __uint_as_float(ag[4 * jj + 2]), __uint_as_float(ag[4 * jj + 3]), bg.z, bg.w);
+            fadd2(a0, a1, av[4 * jj], av[4 * jj + 1], ba.x, ba.y);
+            fadd2(a2, a3, av[4 * jj + 2], av[4 * jj + 3], ba.z, ba.w);
+            fadd2(g0, g1, ag[4 * jj], ag[4 * jj + 1], bg.x, bg.y);
+            fadd2(g2, g3, ag[4 * jj + 2], ag[4 * jj + 3], bg.z, bg.w);
             gelu_erf_f2(g0, g1, y0, y1);
             gelu_erf_f2(g2, g3, y2, y3);
             fmul2(v[4 * jj], v[4 * jj + 1], a0, a1, y0, y1);
@@ -667,53 +664,41 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     }
     if (lane == 0) bulk_wait_read<0>();     // staging tiles must outlive the bulk stores' reads
     __syncwarp();
-    tc_fence_before();
-    if (p.dbg && threadIdx.x == 64) {
+    if (p.dbg && threadIdx.x == 0) {
       long long* d = p.dbg + 8LL * ((static_cast<long long>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
       d[0] = t_start; d[1] = t_setup; d[2] = t_acc; d[3] = clock64();
     }
   }
   if constexpr (PAIR) cluster_sync_all();     // neither CTA may retire while the other can still signal it
-  else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_pair(tmem_base, TMEM_COLS);
-    else tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
-template <int BN, int STAGES, int EW, bool PAIR = false, int KSUB = 1>
+template <int BN, int STAGES, bool PAIR>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const CUtensorMap& tr,
            const GemmParams& p, dim3 grid, cudaStream_t st) {
-  constexpr int smem = STAGES * KSUB * (A_SUB_BYTES + (PAIR ? BN / 2 : BN) * BK * 2) + 1024 + 512;
+  constexpr int smem = GemmSmem<BN, STAGES>::TOTAL;
   static_assert(smem <= 227 * 1024, "pipeline does not fit in shared memory");
+  static_assert((2 * STAGES + 2 * EW) * 8 + 8 <= 512, "barriers do not fit");
   static bool configured = false;
   if (!configured) {
-    DBIR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, EW, PAIR, KSUB>,
+    DBIR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, PAIR>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
-  DBIR_CHECK_CUDA(dbir_launch_cluster(gemm_tc_kernel<BN, STAGES, EW, PAIR, KSUB>, grid, dim3(64 + 32 * EW), smem, st,
+  DBIR_CHECK_CUDA(dbir_launch_cluster(gemm_tc_kernel<BN, STAGES, PAIR>, grid, dim3(GEMM_THREADS), smem, st,
                                       PAIR ? 2u : 1u, ta, tb, to, tr, p));
   return 0;
 }
 
-// Tile width, CTA pairing and split-K factor from a cost model in SM cycles, calibrated on B200
-// with the per-CTA clock64 stamps (tools/gpu_pair_timeline.py, profiles/r01_probes.txt):
-//   * one 64-wide k-block costs max(MMA time, loop overhead): the MMAs take ~2*BN cycles
-//     (128 x BN x 64 at 128 x 256 x 16 per 128 cycles), the producer / issue loops ~520 cycles per
-//     stage iteration (barrier, TMA-issue and commit latencies) -> ~290 per k-block with two
-//     k-blocks per stage (KSUB = 2);
-//   * two CTAs on one SM share its tensor pipe but hide each other's overhead and epilogue;
-//   * epilogue ~1500 + 28*BN cycles with 8 warps, ~500 + 55*BN with 4; split-K adds a workspace
-//     round trip; CTAs are spread over `sms` SMs, a partial last wave costs a full one.
+// Tile width, CTA pairing and split-K factor from a cost model in SM cycles. Every kernel of the
+// family runs one CTA per SM (two warpgroups of register accumulators and a ~200 KB stage ring):
+//   * one 64-wide k-block costs max(MMA time, pipeline overhead): 128 x BN x 64 MACs at the dense
+//     16-bit rate of 2048 MACs per cycle per SM take 4*BN cycles; a stage round trip (barrier wait,
+//     wgmma issue, release) ~200 cycles;
+//   * a CTA pair loads half of B per CTA (multicast): less L2 traffic per k-block, more set-up;
+//   * epilogue ~1200 + 24*BN cycles; split-K adds a workspace round trip; CTAs are spread over `sms`
+//     SMs, a partial last wave costs a full one.
+// The first call of each problem signature replaces this estimate with a measurement (see below).
 struct TilePlan { int bn, splits, kb_per_split, pair; };
-
-__host__ int plan_ksub(int bn, int pair, bool wide) {
-  if (pair) return (bn == 256 && !wide) ? 1 : 2;
-  if (bn == 256) return 1;
-  return (wide || bn <= 64) ? 2 : 1;
-}
 
 struct PlanQuery {
   int m_tiles, N, num_kb, geglu, forced_bn, split_req, pair_req;
@@ -725,13 +710,10 @@ template <typename F>
 void for_each_plan(const PlanQuery& q, F f) {
   const int cands[5] = {256, 160, 128, 64, 32};
   const int sms = dbir_sm_count();
-  // CTA pairs (cta_group::2): DBIR_GEMM_PAIR = 0 never, 1 whenever the shape allows, unset: free choice
+  // CTA pairs (2-CTA clusters sharing B): DBIR_GEMM_PAIR = 0 never, 1 whenever the shape allows, unset: free choice
   static const int pair_env = [] { const char* e = getenv("DBIR_GEMM_PAIR"); return e ? atoi(e) : -1; }();
   const int pair_mode = q.pair_req == 1 ? 1 : q.pair_req == 2 ? 0 : pair_env;
   const bool can_pair = pair_mode != 0 && !(q.m_tiles & 1);
-  // experiment switch (off: wide tiles only when they divide N): SS-mode MMAs run at 75-80 % of peak
-  // only for N = 256, so a ragged last tile can still pay for N = 640 / 1920
-  static const int ragged_wide = [] { const char* e = getenv("DBIR_GEMM_RAGGED_WIDE"); return e ? atoi(e) : 0; }();
   for (int i = 0; i < 10; ++i) {
     const int bn = cands[i % 5];
     const int pair = 1 - i / 5;
@@ -740,7 +722,7 @@ void for_each_plan(const PlanQuery& q, F f) {
     if (q.forced_bn > 0 && bn != q.forced_bn) continue;
     if (q.forced_bn <= 0) {
       if (q.geglu && bn < 64) continue;
-      if (bn > 64 && q.N % bn != 0 && !(ragged_wide && q.N > bn)) continue;   // ragged N only with the narrow tiles
+      if (bn > 64 && q.N % bn != 0) continue;                          // ragged N only with the narrow tiles
     }
     const long long tiles = static_cast<long long>(q.m_tiles) * ((q.N + bn - 1) / bn);
     for (int s = 1; s <= 16; ++s) {
@@ -748,27 +730,18 @@ void for_each_plan(const PlanQuery& q, F f) {
         if (q.split_req == 1 || q.geglu || q.ws_floats_avail <= 0) break;
         if (q.num_kb / s < 6) break;
         if (tiles > 16384 || tiles * s * 128LL * bn > q.ws_floats_avail) break;
-        if (tiles * (s - 1) >= 2LL * sms) break;       // already more than two CTAs per SM without it
+        if (tiles * (s - 1) >= 2LL * sms) break;       // already two waves without it
       }
       if (q.split_req > 1 && s != q.split_req) continue;
       const int kbs = (q.num_kb + s - 1) / s;
       if (static_cast<long long>(kbs) * (s - 1) >= q.num_kb) continue;   // an empty split
       const long long ctas = tiles * s;
-      const bool wide = ctas <= sms;                       // one CTA per SM, 8 epilogue warps
-      const bool two = !wide && (bn <= 160 || pair);       // 4 epilogue warps, two CTAs per SM
-      const int ksub = plan_ksub(bn, pair, wide);
-      double ovh = ksub == 2 ? 290.0 : 520.0;
-      if (pair) ovh *= 0.92;
-      const double mma = 2.0 * bn;
-      const long long slots = static_cast<long long>(sms) * (two ? 2 : 1);
-      const double waves = static_cast<double>((ctas + slots - 1) / slots);
-      double conc = 1.0;                                   // CTAs sharing one tensor pipe
-      if (two) conc = ctas >= 2LL * sms ? 2.0 : static_cast<double>(ctas) / sms;
-      const double iters = static_cast<double>((kbs + ksub - 1) / ksub) * ksub;
-      const double main = iters * (ovh > conc * mma ? ovh : conc * mma);
-      double epi = two ? 500.0 + 55.0 * bn : 1500.0 + 28.0 * bn;
+      const double waves = static_cast<double>((ctas + sms - 1) / sms);
+      const double mma = 4.0 * bn;
+      const double ovh = pair ? 180.0 : 200.0;
+      const double main = kbs * (ovh > mma ? ovh : mma) * (pair ? 0.97 : 1.0);
+      double epi = 1200.0 + 24.0 * bn;
       if (s > 1) epi += 30.0 * bn + 6.0 * bn * s;
-      if (two) epi *= 0.5;
       f(TilePlan{bn, s, kbs, pair}, waves * (2500.0 + (pair ? 900.0 : 0.0) + main + epi));
     }
   }
@@ -818,7 +791,7 @@ struct TuneScratch {
   void* out = nullptr; size_t out_cap = 0;
   void* part = nullptr; size_t part_cap = 0;
   void* flush = nullptr;
-  static constexpr size_t FLUSH_BYTES = 192u << 20;     // > the 126 MB L2
+  static constexpr size_t FLUSH_BYTES = 128u << 20;     // > 2.5x the 50 MB L2
   cudaEvent_t ev[3][2] = {};
   bool ready = false;
 };
@@ -1082,33 +1055,20 @@ int gemm_impl(const dbir_gemm_args* a, cudaStream_t st, const TilePlan* forced) 
     if (dbir_make_tmap(&tb, a->b, 2, dims, strides, box, 2, 1)) return -3;
   }
   dim3 grid(m_tiles, (a->N + bn - 1) / bn, plan.splits);
-  // <= one CTA per SM anyway -> 8 epilogue warps and a deeper pipeline; else two CTAs per SM
-  static const int wide_mode = [] { const char* e = getenv("DBIR_GEMM_WIDE"); return e ? atoi(e) : -1; }();
-  const bool wide = wide_mode >= 0 ? wide_mode != 0
-                                   : static_cast<long long>(grid.x) * grid.y * grid.z <= dbir_sm_count();
-  // <BN, STAGES, EW, PAIR, KSUB>: EW == 4 kernels run two CTAs per SM (<= ~104 KB of stages each)
-#define DBIR_GO(BN_, ST_, EW_, PAIR_, KS_) return launch<BN_, ST_, EW_, PAIR_, KS_>(ta, tb, to, tr, p, grid, st)
-  if (plan.pair) {
-    switch (bn) {
-      case 64:  if (wide) DBIR_GO(64, 4, 8, true, 2);  else DBIR_GO(64, 2, 4, true, 2);
-      case 128: if (wide) DBIR_GO(128, 4, 8, true, 2); else DBIR_GO(128, 2, 4, true, 2);
-      case 160: if (wide) DBIR_GO(160, 4, 8, true, 2); else DBIR_GO(160, 2, 4, true, 2);
-      case 256: if (wide) DBIR_GO(256, 3, 8, true, 2); else DBIR_GO(256, 3, 4, true, 1);
-      default:
-        dbir_set_error("dbir_gemm: unsupported paired tile width %d", bn);
-        return -2;
-    }
-  }
+  // <BN, STAGES, PAIR>: stage rings of 160-224 KB, one CTA per SM
+#define DBIR_GO(BN_, ST_) return plan.pair ? launch<BN_, ST_, true>(ta, tb, to, tr, p, grid, st) \
+                                           : launch<BN_, ST_, false>(ta, tb, to, tr, p, grid, st)
   switch (bn) {
-    case 32:  if (wide) DBIR_GO(32, 4, 8, false, 2);  else DBIR_GO(32, 2, 4, false, 2);
-    case 64:  if (wide) DBIR_GO(64, 4, 8, false, 2);  else DBIR_GO(64, 2, 4, false, 2);
-    case 128: if (wide) DBIR_GO(128, 3, 8, false, 2); else DBIR_GO(128, 3, 4, false, 1);
-    case 160: if (wide) DBIR_GO(160, 3, 8, false, 2); else DBIR_GO(160, 3, 4, false, 1);
-    case 256: DBIR_GO(256, 4, 8, false, 1);
-    default:
-      dbir_set_error("dbir_gemm: unsupported tile width %d", bn);
-      return -2;
+    case 32:  if (plan.pair) break; return launch<32, 8, false>(ta, tb, to, tr, p, grid, st);
+    case 64:  DBIR_GO(64, 8);
+    case 128: DBIR_GO(128, 6);
+    case 160: DBIR_GO(160, 6);
+    case 256: DBIR_GO(256, 4);
+    default: break;
   }
+#undef DBIR_GO
+  dbir_set_error("dbir_gemm: unsupported tile width %d (pair %d)", bn, plan.pair);
+  return -2;
 }
 }  // namespace
 

@@ -160,8 +160,8 @@ __device__ __forceinline__ void fin_accumulate(const float* __restrict__ base, i
 
 // SPLIT > 1: a (SPLIT,1,1) cluster shares one (group, image); every CTA reduces an interleaved share of the
 // partial pairs, the shares meet in CTA 0 through distributed shared memory in rank order (deterministic).
-// A VAE layer at 512^2 has 8192 row slots x 4 channels per group: one CTA per group took 91 us there
-// (ncu: 8.4 MB read by 32 CTAs), and 16x that at 2048^2.
+// A VAE layer at 512^2 has 8192 row slots x 4 channels per group: one CTA per group would read its
+// 8.4 MB with only 32 CTAs in the grid, and 16x that at 2048^2.
 template <int SPLIT>
 __global__ void __launch_bounds__(FIN_THREADS)
 gn_finalize_kernel(const float* __restrict__ p1, int slots1, int c1, const float* __restrict__ p2,

@@ -18,7 +18,7 @@ void dbir_set_error(const char* fmt, ...) {
 
 extern "C" const char* dbir_last_error(void) { return g_err; }
 extern "C" const char* dbir_version(void) {
-  return "diffbir_b200 0.1 (sm_100a; tcgen05/TMEM/TMA)";
+  return "diffbir_b200 0.1 (sm_90a; wgmma/TMA)";
 }
 extern "C" int dbir_operand_kind(void) { return DBIR_OPERAND_KIND; }
 extern "C" int dbir_pdl_enabled(void) {
@@ -32,7 +32,7 @@ extern "C" int dbir_sm_count(void) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-      sms = 148;
+      sms = 132;
   }
   return sms;
 }

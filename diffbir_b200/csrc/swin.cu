@@ -10,8 +10,8 @@
 // staged in shared memory as fp32 and read as warp-wide broadcasts (LDS.128, conflict-free);
 // the query row, the 64 scores, the softmax and the 30 outputs stay in registers. HBM-/latency-
 // bound (6 MB of qkv + 2 MB of output per 512^2 image, 0.19 GFLOP): the grid of
-// windows x heads = 384 CTAs at 512^2 fills the 148 SMs where one CTA per window (64 CTAs with
-// two query rows per lane) left most of them idle (136 us -> see profiles/r02_*).
+// windows x heads = 384 CTAs at 512^2 fills the 132 SMs where one CTA per window (64 CTAs with
+// two query rows per lane) leaves most of them idle.
 #include "common.cuh"
 #include "../../include/diffbir_b200.h"
 

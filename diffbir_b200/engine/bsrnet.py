@@ -1,4 +1,4 @@
-"""RRDBNet (BSRNet stage-1 cleaner of the v2 recipe) on the sm_100a kernels.
+"""RRDBNet (BSRNet stage-1 cleaner of the v2 recipe) on the sm_90a kernels.
 
 Replaces RRDBNet.forward (reference model/bsrnet.py:89-104): conv_first, 23 RRDB blocks of three
 5-convolution residual dense blocks (:36-73), trunk conv + skip, two nearest-2x + conv + LeakyReLU

@@ -1,4 +1,4 @@
-"""ControlNet + ControlledUnetModel forward on the sm_100a kernels.
+"""ControlNet + ControlledUnetModel forward on the sm_90a kernels.
 
 Replaces ControlLDM.forward (reference model/cldm.py:160-172), i.e. ControlNet.forward
 (model/controlnet.py:314-328) and ControlledUnetModel.forward (model/controlnet.py:18-47),
@@ -168,7 +168,7 @@ class CldmEngine:
         self._ts_key = None
         self._part = {}                  # fp32 activation data_ptr -> (GN partial-sum buffer, slots)
         self._wseq, self._wpos = {}, {}  # per-stream weight sequence of the forward (L2 prefetch lookahead)
-        self.prefetch_weights = False    # measured: no gain on B200 (7.53 vs 7.45 ms per forward), kept opt-in
+        self.prefetch_weights = False    # opt-in: L2 prefetch of the next layers' weights during a GEMM
         self.fuse_gn_stats = True
         # Batch-invariant kernel plans: no split-K, whole attention tiles per CTA. Every sample's result
         # then has the same bits whatever batch it runs in (tiled sampling: sharded == single rank) and

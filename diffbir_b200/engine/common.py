@@ -108,9 +108,8 @@ def pack_linear(w: torch.Tensor, device, k_pad: int = 0) -> torch.Tensor:
 def geglu_tile(c: int) -> int:
     """GEMM tile width used for the GEGLU projection of a width-c transformer block (the weights are packed
     per tile as [values | gates], so it is fixed at load time)."""
-    # 256-wide tiles (128 values + 128 gates, run as CTA pairs): at large batch the projection is bound by
-    # L2 -> SM operand traffic, which a 256 x 256 pair tile halves against 128 x 128 (B200, 28 tile-forwards:
-    # the three GEGLU shapes 4.1 -> 3.6 ms per forward; batch 2: 5.80 -> 5.65 ms). DBIR_GEGLU_TILE overrides.
+    # 256-wide tiles (128 values + 128 gates): at large batch the projection is bound by L2 -> SM operand
+    # traffic, which a 256-wide tile (and a CTA pair sharing it) cuts against 128-wide ones. DBIR_GEGLU_TILE overrides.
     forced = int(os.environ.get("DBIR_GEGLU_TILE", "0"))       # A/B switch: 64 | 128 | 256
     for bn in ((forced,) if forced else ()) + (256, 128, 64):
         if (8 * c) % bn == 0:

@@ -1,4 +1,4 @@
-"""SCUNet (Swin-Conv-UNet, the v2 blind-denoising stage-1 cleaner) on the sm_100a kernels.
+"""SCUNet (Swin-Conv-UNet, the v2 blind-denoising stage-1 cleaner) on the sm_90a kernels.
 
 Replaces SCUNet.forward (reference model/scunet.py:221-243): head conv, three down stages, body, three up
 stages of ConvTransBlocks (:126-156) joined by 2x2 stride-2 convs / transposed convs, tail conv.

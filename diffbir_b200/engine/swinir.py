@@ -1,4 +1,4 @@
-"""Stage-1 SwinIR forward on the sm_100a kernels.
+"""Stage-1 SwinIR forward on the sm_90a kernels.
 
 Replaces SwinIR.forward / forward_features (reference model/swinir.py:856-894, 841-854), RSTB
 (:487-488), SwinTransformerBlock.forward (:245-285) and WindowAttention.forward (:120-151)

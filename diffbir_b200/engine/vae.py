@@ -1,4 +1,4 @@
-"""AutoencoderKL decode / encode on the sm_100a kernels.
+"""AutoencoderKL decode / encode on the sm_90a kernels.
 
 Replaces AutoencoderKL.decode -> Decoder.forward (reference model/vae.py:579-582, 526-559)
 and AutoencoderKL.encode -> Encoder.forward (vae.py:573-577, 347-371) for the SD VAE of

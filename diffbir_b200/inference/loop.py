@@ -82,7 +82,7 @@ def load_checkpoint(path: str) -> dict:
 def check_supported(args: Namespace) -> None:
     """Everything this package cannot honour is refused here, before any model is built."""
     if args.device != "cuda":
-        raise NotImplementedError(f"--device {args.device}: the engines are CUDA (sm_100a) only, there is no CPU path")
+        raise NotImplementedError(f"--device {args.device}: the engines are CUDA (sm_90a) only, there is no CPU path")
     if args.sampler not in SUPPORTED_SAMPLERS:
         raise NotImplementedError(f"--sampler {args.sampler}: not one of {SUPPORTED_SAMPLERS}")
     if args.captioner != "none":

@@ -1,7 +1,7 @@
 """ControlLDM — drop-in counterpart of the reference's diffbir.model.ControlLDM
 (model/cldm.py:20-210): same constructor arguments (the YAML `params` of
 configs/inference/cldm.yaml), same checkpoint loaders, same methods and the mutable
-`control_scales` list the pipeline sets per call — backed by the sm_100a kernel engines
+`control_scales` list the pipeline sets per call — backed by the sm_90a kernel engines
 instead of nn.Modules.  There is no eager / CPU path: every method needs the CUDA library.
 """
 from __future__ import annotations
@@ -157,7 +157,7 @@ class ControlLDM:
                    tile_size: int = -1) -> torch.Tensor:
         self._build()
         if tiled:
-            raise NotImplementedError("tiled VAE (utils/tilevae) is outside the B200 hot path: 180 GB HBM")
+            raise NotImplementedError("tiled VAE (utils/tilevae) is outside the hot path: the VAE engines run un-tiled")
         image = image.to(self.device, torch.float32).contiguous()
         sv = self._sharded_vae(image.shape[2], image.shape[3])
         m = sv.encode_moments(image) if sv is not None else self.vae.encode_moments(image)
@@ -171,7 +171,7 @@ class ControlLDM:
     def vae_decode(self, z: torch.Tensor, tiled: bool = False, tile_size: int = -1) -> torch.Tensor:
         self._build()
         if tiled:
-            raise NotImplementedError("tiled VAE (utils/tilevae) is outside the B200 hot path: 180 GB HBM")
+            raise NotImplementedError("tiled VAE (utils/tilevae) is outside the hot path: the VAE engines run un-tiled")
         z = (z / self.scale_factor).to(self.device, torch.float32).contiguous()
         sv = self._sharded_vae(8 * z.shape[2], 8 * z.shape[3])
         return sv.decode(z) if sv is not None else self.vae.decode(z)

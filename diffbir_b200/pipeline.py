@@ -80,7 +80,7 @@ class Pipeline:
         """pipeline.py:71-233."""
         bs, _, h0, w0 = cond_img.shape
         cond_img = pad_to_multiples_of(cond_img, multiple=64 if not vae_encoder_tiled and not cldm_tiled else 8)
-        # Tiled-VAE itself is outside the path (180 GB of HBM), but the reference switches it off for inputs smaller than
+        # Tiled-VAE itself is outside the path (the VAE engines run un-tiled), but the reference switches it off for inputs smaller than
         # a tile (pipeline.py:106-110, 219-223) and then only the padding rule above differs: that branch is honoured.
         if vae_encoder_tiled and (cond_img.size(2) < vae_encoder_tile_size or cond_img.size(3) < vae_encoder_tile_size):
             print("[VAE Encoder]: the input size is tiny and unnecessary to tile.")
@@ -89,7 +89,7 @@ class Pipeline:
             print("[VAE Decoder]: the input size is tiny and unnecessary to tile.")
             vae_decoder_tiled = False
         if vae_encoder_tiled or vae_decoder_tiled:
-            raise NotImplementedError("tiled VAE is outside the B200 hot path (180 GB HBM per GPU): the VAE engines run un-tiled")
+            raise NotImplementedError("tiled VAE is outside the hot path: the VAE engines run un-tiled")
         # ranks that cooperate on this job (sharded tiles or batch units) also shard the VAE by image rows
         import torch.distributed as dist
         coop = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and (cldm_tiled or self.shard_batch)
@@ -216,7 +216,7 @@ class SwinIRPipeline(Pipeline):
     def apply_cleaner(self, lq: torch.Tensor, tiled: bool, tile_size: int, tile_stride: int) -> torch.Tensor:
         """pipeline.py:371-397. Un-tiled: resize the short edge to >= 512 first, pad to x64, crop.
         Tiled: Gaussian-blended `tile_size` windows through make_tiled_fn, resize afterwards (the
-        reference's order in each branch). 180 GB of HBM rarely need the tiled branch; it is kept for
+        reference's order in each branch). The un-tiled branch fits one GPU's memory; the tiled one is kept for
         parity of results with runs of the reference that used it."""
         if tiled and (lq.size(2) < tile_size or lq.size(3) < tile_size):
             print("[SwinIR]: the input size is tiny and unnecessary to tile.")

@@ -1,4 +1,4 @@
-/* diffbir_b200 — C ABI of libdiffbir_b200.so (hand-written sm_100a kernels).
+/* diffbir_b200 — C ABI of libdiffbir_b200.so (hand-written sm_90a kernels).
  *
  * This is the drop-in boundary for the DiffBIR restoration hot path. The reference
  * (XPixelGroup/DiffBIR) has no FFI: every op below replaces a PyTorch library call made
@@ -27,7 +27,7 @@ const char* dbir_last_error(void);
 int dbir_operand_kind(void);          /* 1 = fp16 operands, 0 = bf16 operands */
 int dbir_sm_count(void);              /* SMs of the current device (cached) */
 
-/* ---- tcgen05 GEMM / implicit 3x3 convolution --------------------------------------
+/* ---- wgmma GEMM / implicit 3x3 convolution --------------------------------------
  * out = residual + alpha * act(A * B^T + bias + rowvec)          (GEGLU: a * gelu(g))
  * Replaces nn.Linear (attention.py:22,35-42,67-73,310,331; swinir.py:21-31,104,106),
  * nn.Conv2d 3x3 / 1x1 (unet.py:67,99,149-153,173-188; controlnet.py:309-312;
@@ -64,7 +64,7 @@ typedef struct dbir_gemm_args {
                            partial tiles); NULL disables split-K. Summation order is fixed. */
   int64_t splitk_ws_bytes;
   int32_t split_k;      /* 0 = auto, 1 = off, n > 1 = force n splits */
-  int32_t cta_pair;     /* CTA pairs (cta_group::2, M=256 MMAs): 0 = auto, 1 = whenever the tile count is even, 2 = never */
+  int32_t cta_pair;     /* CTA pairs (2-CTA clusters sharing the B tile by TMA multicast): 0 = auto, 1 = whenever the tile count is even, 2 = never */
   void* debug_stamps;   /* optional int64 [ctas][8] clock64 stamps (start, setup, acc ready, end) */
   void* gn_partials;    /* optional fp32 [img][dbir_gemm_gn_slots()][N][2]: per 32-row-slot column sums and
                            sums of squares of the OUTPUT (fused GroupNorm statistics; see dbir_gn_finalize) */
@@ -86,7 +86,7 @@ int dbir_gemm_model_plan(int32_t m_tiles, int32_t N, int32_t num_kb, int32_t geg
                          int32_t split_k, int32_t cta_pair, int64_t ws_floats, int32_t* out);
 void dbir_gemm_clear_plans(void);         /* forget every cached plan */
 
-/* ---- flash attention, head_dim 64 (tcgen05) ------------------------------------------
+/* ---- flash attention, head_dim 64 (wgmma) --------------------------------------------
  * out[b, i, h*64 + :] = softmax_j(q_h[i] . k_h[j] / 8) v_h[j]; q/k/v/out are op16 matrices
  * [batch, s, ld*] whose first heads*64 columns (from the given base pointer) hold the heads.
  * Replaces F.scaled_dot_product_attention and the head split/merge copies in
@@ -205,16 +205,6 @@ int dbir_tile_gather(const float* full, int32_t b, int32_t c, int32_t h, int32_t
 int dbir_tile_blend(const float* tiles, int32_t b, int32_t c, int32_t h, int32_t w,
                     const int32_t* coords, int32_t ntiles, int32_t tile, const float* weights,
                     float* out, void* stream);
-
-/* ---- calibration probes: only in builds made with -DDBIR_DEBUG_PROBES (python -m diffbir_b200.build
- * --tag=probes -DDBIR_DEBUG_PROBES -DDBIR_ATTN_PROBE, loaded with DBIR_LIB_TAG=probes); the product libraries
- * do not export them.
- * Cycles for `iters` back-to-back 128 x n x 16 tcgen05 MMAs (one CTA) into out_cycles[0] (int64). */
-#ifdef DBIR_DEBUG_PROBES
-void dbir_debug_attn_stamps(void* buf);   /* per-CTA clock64 sums of later attention launches -> buf [ctas][8] int64; NULL = off */
-int dbir_debug_mma_rate(int32_t n, int32_t b_mn_major, int32_t iters, int32_t a_in_tmem, void* out_cycles,
-                        void* stream);
-#endif
 
 /* ---- fused output epilogue -------------------------------------------------------------
  * fixed = high_freq((sample + 1) / 2) + low_freq(style): wavelet_reconstruction (utils/common.py:29-77,

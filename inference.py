@@ -1,4 +1,4 @@
-"""Command line of the reference's inference.py (same flags, same meaning) on the B200 engines.
+"""Command line of the reference's inference.py (same flags, same meaning) on the H100 engines.
 
   python inference.py --task sr --upscale 4 --version v2.1 --sampler spaced --steps 50 \
       --captioner none --pos_prompt '' --neg_prompt 'low quality, blurry' --cfg_scale 4.0 \
@@ -101,7 +101,7 @@ def set_seed(seed: int) -> None:
 def main(argv=None) -> None:
     args = parse_args(argv)
     if args.device == "cuda" and not torch.cuda.is_available():
-        raise SystemExit("inference.py needs a CUDA device (sm_100a): there is no CPU fallback for the engines")
+        raise SystemExit("inference.py needs a CUDA device (sm_90a): there is no CPU fallback for the engines")
     set_seed(args.seed)
     from diffbir_b200.inference import BFRInferenceLoop, BIDInferenceLoop, BSRInferenceLoop, CustomInferenceLoop
     loops = {"sr": BSRInferenceLoop, "face": BFRInferenceLoop, "denoise": BIDInferenceLoop}

@@ -23,6 +23,7 @@ from _ref_import import use_reference  # noqa: E402
 use_reference()
 from diffbir_b200 import arch  # noqa: E402
 from diffbir_b200.utils.synth import make_state_dict  # noqa: E402
+from tests.golden_io import save_golden  # noqa: E402
 
 OUT = Path(__file__).resolve().parent
 
@@ -108,8 +109,8 @@ def main():
     out["scunet_y"] = scu(xc)[..., ::2, ::2].numpy()
     print("scunet full", float(np.abs(out["scunet_y"]).mean()), flush=True)
 
-    np.savez_compressed(OUT / "full_config.npz", **out)
-    print("wrote full_config.npz")
+    save_golden(OUT, "full_config", out)
+    print("wrote full_config.npz and its parts")
 
 
 if __name__ == "__main__":

@@ -7,7 +7,7 @@ through the reference's own loaders), 50-step DDIM (eta 0, batched CFG), cfg 4.0
 -> tests/golden/full_pipeline_ddim.npz (the uint8 result). DDIM with eta 0 draws no per-step noise, so the CPU-drawn x_T
 (`torch.manual_seed(231); torch.randn(1, 4, 64, 64)`) is the only randomness and a GPU run can be fed the same one.
 `--oracle` also replays the run through the oracle's restatement of the pipeline and prints the difference (too slow for
-the CPU test suite; the printed lines are committed as profiles/r02_full_pipeline_oracle_vs_reference.log).
+the CPU test suite).
 `--spaced` does the same for configs[1] (50-step spaced sampler, image seed 0); its per-step noise comes from the CPU
 generator, which a GPU run cannot reproduce, so that variant only serves the oracle comparison and writes no fixture;
 `--v21` uses configs/inference/diffusion_v2.1.yaml (v-parameterization, zero terminal SNR) with the cosine CFG ramp.

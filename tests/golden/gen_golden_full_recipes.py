@@ -8,7 +8,6 @@
 each 20 steps, cfg 4.0, seed 231, all networks at the sizes of configs/inference/*.yaml with seeded random-init weights.
 The reference's own pipeline runs first; then this package's pipeline + sampler classes run with the oracle networks
 plugged in where the kernel engines sit (the harness of tests/test_oracle_golden.py), and the uint8 images are compared.
-Printed lines are committed as profiles/r02_full_recipes_host_code_vs_reference.log.
 """
 import contextlib
 import sys

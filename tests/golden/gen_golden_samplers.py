@@ -16,8 +16,10 @@ from pathlib import Path
 import numpy as np
 import torch
 
+sys.path.insert(0, str(Path(__file__).resolve().parents[2]))
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 from _ref_import import use_reference  # noqa: E402
+from tests.golden_io import save_golden  # noqa: E402
 
 use_reference()
 OUT = Path(__file__).resolve().parent
@@ -88,8 +90,8 @@ def main():
             z = fns[solver](den, x0.clone(), s.sigmas, disable=True, eta=HP["eta"], s_noise=HP["s_noise"],
                             noise_sampler=seeded_noise(11))
             out[f"sde_{pname}_{solver}"] = z.numpy()
-    np.savez_compressed(OUT / "samplers.npz", **out)
-    print("wrote", OUT / "samplers.npz", len(out), "arrays")
+    save_golden(OUT, "samplers", out)
+    print("wrote", OUT / "samplers.npz", "and its parts,", len(out), "arrays")
 
 
 if __name__ == "__main__":

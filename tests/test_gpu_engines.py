@@ -14,6 +14,7 @@ from diffbir_b200 import arch
 from diffbir_b200.utils.synth import make_state_dict
 from tests.gpu_util import no_tf32, psnr, rel_rms, to_dev
 from tests.small_cfg import CN_SMALL, SWIN_SMALL, UNET_SMALL, VAE_SMALL
+from tests.golden_io import load_golden
 
 pytestmark = pytest.mark.gpu
 TOL = 4e-3
@@ -83,7 +84,7 @@ def test_cldm_full_config_vs_oracle(golden_dir):
     modules on the same weights and inputs (tests/golden/full_config.npz, gen_golden_full.py)."""
     from oracle import cldm as ocl
     no_tf32()
-    g = np.load(golden_dir / "full_config.npz")
+    g = load_golden(golden_dir, "full_config")
     eng, usd, csd = _cldm_engine(arch.UNET_CFG, arch.CONTROLNET_CFG, seeds=(1234, 1235))
     gen = torch.Generator().manual_seed(0)
     x = torch.randn(1, 4, 64, 64, generator=gen).repeat(2, 1, 1, 1).cuda()
@@ -120,7 +121,7 @@ def test_vae_full_config_vs_oracle(golden_dir):
     from diffbir_b200.engine.vae import VaeEngine
     from oracle import cldm as ocl
     no_tf32()
-    g = np.load(golden_dir / "full_config.npz")
+    g = load_golden(golden_dir, "full_config")
     sd = make_state_dict(arch.vae_shapes(arch.VAE_CFG), 77)
     eng = VaeEngine(sd, None, "cuda")
     sd_d = to_dev(sd)
@@ -168,7 +169,7 @@ def test_swinir_full_config_vs_oracle(size, golden_dir):
     print(f"swinir {size}: max err / std = {err:.2e}, psnr(peak 1) {psnr(y, ref, 1.0):.1f} dB")
     assert err < 3e-2
     if size == 256:                                            # the reference's own output for this weight / input pair
-        gref = torch.from_numpy(np.load(golden_dir / "full_config.npz")["swinir_y256"]).cuda()
+        gref = torch.from_numpy(load_golden(golden_dir, "full_config")["swinir_y256"]).cuda()
         eg = ((y - gref).abs().max() / gref.std()).item()
         print(f"swinir 256 vs reference fixture: max err / std = {eg:.2e}")
         assert eg < 3e-2
@@ -201,7 +202,7 @@ def test_rrdbnet_full_config_vs_oracle(golden_dir):
     with torch.no_grad():
         ref = ob.rrdbnet_forward(to_dev(sd), x)
     e = rel_rms(y, ref)
-    g = np.load(golden_dir / "full_config.npz")
+    g = load_golden(golden_dir, "full_config")
     st = int(g["rrdb_stride"])
     eg = rel_rms(y[..., ::st, ::st], torch.from_numpy(g["rrdb_y"]).cuda())
     print(f"rrdbnet full: rel rms {e:.2e}, psnr(peak 1) {psnr(y, ref, 1.0):.1f} dB, |y| {ref.abs().mean():.4f}; vs reference fixture {eg:.2e}")
@@ -236,7 +237,7 @@ def test_scunet_full_config_vs_oracle(golden_dir):
     with torch.no_grad():
         ref = osc.scunet_forward(to_dev(sd), x)
     e = rel_rms(y, ref)
-    g = np.load(golden_dir / "full_config.npz")
+    g = load_golden(golden_dir, "full_config")
     st = int(g["scunet_stride"])
     eg = rel_rms(y[..., ::st, ::st], torch.from_numpy(g["scunet_y"]).cuda())
     print(f"scunet full: rel rms {e:.2e}, psnr(peak 1) {psnr(y, ref, 1.0):.1f} dB, |y| {ref.abs().mean():.4f}; vs reference fixture {eg:.2e}")

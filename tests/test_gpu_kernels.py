@@ -272,7 +272,7 @@ def test_sampler_step_and_tiles_bit_exact(L, golden_dir):
                                          (8192, 320, 320, 0), (4000, 320, 320, 160), (1024, 200, 448, 64),
                                          (2048, 1280, 640, 256)])
 def test_gemm_cta_pair_plain(L, M, N, K, fbn):
-    """cta_group::2 path (M=256 MMAs over a 2-CTA cluster): same fp32 result as the single-CTA
+    """CTA-pair path (2-CTA cluster sharing the B tile by TMA multicast): same fp32 result as the single-CTA
     path up to accumulation order (identical here: same k order), and vs the fp32 reference."""
     dt = L.operand_dtype()
     a, b = rnd(M, K, seed=1).to(dt), rnd(N, K, seed=2, scale=K ** -0.5).to(dt)

@@ -9,6 +9,7 @@ from oracle import cldm as ocl
 from oracle import sampling as osm
 from oracle import swinir as osw
 from tests.small_cfg import CN_SMALL, SWIN_SMALL, UNET_SMALL, VAE_SMALL
+from tests.golden_io import load_golden
 
 
 def close(a, b, rtol=2e-5):
@@ -320,7 +321,7 @@ def test_full_config_oracle_matches_reference(golden_dir):
     GPU tests (tests/golden/gen_golden_full.py): the reference == oracle == CUDA chain is closed at full width too."""
     from oracle import bsrnet as ob
     from oracle import scunet as osc
-    g = np.load(golden_dir / "full_config.npz")
+    g = load_golden(golden_dir, "full_config")
     res = {}
     with torch.no_grad():
         usd = make_state_dict(arch.unet_shapes(arch.UNET_CFG), 1234, arch.is_zero_init)
