@@ -1,8 +1,6 @@
 """In-tree build of libdiffbir_b200.so (sm_90a only; nvcc cross-compiles without a GPU).
 
-    python -m diffbir_b200.build [--bf16] [--force] [-DNAME ...]
-
-Extra -D switches (also from $DBIR_BUILD_DEFS) select compile-time experiments.
+    python -m diffbir_b200.build [--bf16] [--force] [-v]
 
 Objects go to diffbir_b200/csrc/_build/, the library to diffbir_b200/libdiffbir_b200.so
 (git-ignored). --bf16 builds the bf16-operand
@@ -36,15 +34,13 @@ def _digest(paths, extra):
     return h.hexdigest()
 
 
-def build_library(bf16: bool = False, force: bool = False, verbose: bool = False, extra_defs=(), tag: str = "") -> Path:
-    """tag: experiment builds (extra -D switches) go to libdiffbir_b200_<tag>.so / csrc/_build_<tag>/ and
-    are loaded with DBIR_LIB_TAG=<tag>; the product libraries are the untagged fp16 / bf16 ones."""
+def build_library(bf16: bool = False, force: bool = False, verbose: bool = False) -> Path:
     srcs = sorted(CSRC.glob("*.cu"))
     hdrs = sorted(CSRC.glob("*.cuh")) + sorted((HERE.parent / "include").glob("*.h"))
-    defs = (["-DDBIR_OPERAND_BF16"] if bf16 else []) + list(extra_defs) + os.environ.get("DBIR_BUILD_DEFS", "").split()
-    bdir = CSRC / (f"_build_{tag}" if tag else "_build_bf16" if bf16 else "_build")
+    defs = ["-DDBIR_OPERAND_BF16"] if bf16 else []
+    bdir = CSRC / ("_build_bf16" if bf16 else "_build")
     bdir.mkdir(exist_ok=True)
-    out = HERE / f"libdiffbir_b200_{tag}.so" if tag else OUT_BF16 if bf16 else OUT
+    out = OUT_BF16 if bf16 else OUT
     stamp = bdir / "stamp.txt"
     dig = _digest(srcs + hdrs, ARCH + FLAGS + defs)
     if out.exists() and stamp.exists() and stamp.read_text() == dig and not force:
@@ -80,8 +76,5 @@ def build_library(bf16: bool = False, force: bool = False, verbose: bool = False
 
 
 if __name__ == "__main__":
-    tags = [a.split("=", 1)[1] for a in sys.argv[1:] if a.startswith("--tag=")]
-    p = build_library(bf16="--bf16" in sys.argv, force="--force" in sys.argv,
-                      verbose="-v" in sys.argv, extra_defs=[a for a in sys.argv[1:] if a.startswith("-D")],
-                      tag=tags[0] if tags else "")
+    p = build_library(bf16="--bf16" in sys.argv, force="--force" in sys.argv, verbose="-v" in sys.argv)
     print(p)

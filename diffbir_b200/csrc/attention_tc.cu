@@ -16,7 +16,6 @@
 // Two CTAs are resident per SM (80 KB shared memory each).
 #include "common.cuh"
 #include "../../include/diffbir_b200.h"
-#include <stdlib.h>
 
 namespace {
 
@@ -313,9 +312,8 @@ int attn_plan(int batch, int heads, int sq, int skv, int* parts_max) {
   const long long tiles = static_cast<long long>(batch) * heads * q_tiles;
   const long long slots = static_cast<long long>(CTAS_PER_SM) * dbir_sm_count();
   *parts_max = 0;
-  static const int sk_mode = [] { const char* e = getenv("DBIR_ATTN_STREAMK"); return e ? atoi(e) : 1; }();
   // (the ticket array holds 16384 tiles; such grids are many waves deep and need no balancing)
-  if (!sk_mode || n_steps < 8 || tiles * n_steps < slots * 4 || tiles > 16384) return static_cast<int>(tiles);
+  if (n_steps < 8 || tiles * n_steps < slots * 4 || tiles > 16384) return static_cast<int>(tiles);
   const long long waves = (tiles + slots - 1) / slots;
   // a single, partly filled wave is left alone: its CTAs mostly have an SM to themselves
   if (waves < 2 || static_cast<double>(tiles) / static_cast<double>(waves * slots) >= 0.8) return static_cast<int>(tiles);
@@ -336,10 +334,10 @@ extern "C" int64_t dbir_attention_ws_bytes(int32_t batch, int32_t heads, int32_t
   return ATTN_TICKET_BYTES + tiles * parts_max * TQ * WS_ROW * 4;
 }
 
-extern "C" int dbir_attention_sk(const void* q, const void* k, const void* v, void* out,
-                                 int32_t batch, int32_t heads, int32_t sq, int32_t skv,
-                                 int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo,
-                                 void* ws, int64_t ws_bytes, void* stream) {
+extern "C" int dbir_attention(const void* q, const void* k, const void* v, void* out,
+                              int32_t batch, int32_t heads, int32_t sq, int32_t skv,
+                              int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo,
+                              void* ws, int64_t ws_bytes, void* stream) {
   DBIR_REQUIRE(q && k && v && out, "dbir_attention: null pointer");
   DBIR_REQUIRE(batch > 0 && heads > 0 && sq > 0 && skv > 0, "dbir_attention: bad shape");
   DBIR_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0,
@@ -383,10 +381,4 @@ extern "C" int dbir_attention_sk(const void* q, const void* k, const void* v, vo
     DBIR_CHECK_CUDA(dbir_launch(attn_fwd_kernel<false>, dim3(ctas), dim3(ATTN_THREADS), ATTN_SMEM,
                                 reinterpret_cast<cudaStream_t>(stream), mq, mk, mv, p));
   return 0;
-}
-
-extern "C" int dbir_attention(const void* q, const void* k, const void* v, void* out,
-                              int32_t batch, int32_t heads, int32_t sq, int32_t skv,
-                              int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo, void* stream) {
-  return dbir_attention_sk(q, k, v, out, batch, heads, sq, skv, ldq, ldk, ldv, ldo, nullptr, 0, stream);
 }

@@ -80,13 +80,12 @@ extern "C" int dbir_sm_count(void);
 #ifdef __CUDACC__
 // ---------------------------------------------------------------------------
 // Programmatic dependent launch (PDL): every kernel is launched with the programmatic-stream-serialization
-// attribute (on by default, DBIR_PDL=0 turns it off); each one calls pdl_trigger() at entry (lets the NEXT
-// kernel's CTAs be scheduled and run their prologue: barrier init, descriptor prefetch) and
+// attribute; each one calls pdl_trigger() at entry (lets the NEXT kernel's CTAs be scheduled and run
+// their prologue: barrier init, descriptor prefetch) and
 // pdl_wait() before touching memory written by its predecessors (griddepcontrol.wait returns when all
 // prerequisite grids completed and flushed). The ~200 KB shared-memory GEMM CTAs cannot co-reside with
 // their successor's CTAs, so there is little to overlap there; the smaller kernels' prologues do overlap.
 // ---------------------------------------------------------------------------
-extern "C" int dbir_pdl_enabled(void);
 template <typename... KArgs, typename... Args>
 inline cudaError_t dbir_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
                                        cudaStream_t st, unsigned cluster_x, Args&&... args) {
@@ -96,12 +95,9 @@ inline cudaError_t dbir_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[2];
-  int n = 0;
-  if (dbir_pdl_enabled()) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  int n = 1;
   if (cluster_x > 1) {
     attr[n].id = cudaLaunchAttributeClusterDimension;
     attr[n].val.clusterDim.x = cluster_x;

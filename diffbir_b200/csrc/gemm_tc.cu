@@ -63,15 +63,10 @@ struct GemmParams {
   int splits, kb_per_split;
   float* ws;
   unsigned int* tickets;
-  long long* dbg;          // optional per-CTA clock64 stamps [ctas][4]: start, setup done, acc ready, end
   // fused GroupNorm statistics of the OUTPUT tensor: per (image, 32-row slot, channel) sum / sum of
   // squares over the warp's rows -> stats[(img * nslots + slot) * N + col][2] (fp32 outputs only)
   float* stats;
   int stats_nslots, stats_rows_per_img, stats_slots_x;
-  // L2 prefetch of memory a LATER kernel will stream (the next layers' weights): issued by the
-  // epilogue warps while they wait for the mainloop
-  const char* pf_ptr;
-  long long pf_bytes;
 };
 
 __device__ __forceinline__ float apply_act(float v, int act, float prm) {
@@ -329,8 +324,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   const int tile_lin = blockIdx.y * gridDim.x + blockIdx.x;
   const int kb0 = blockIdx.z * p.kb_per_split;
   const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
-  long long t_start = 0, t_setup = 0, t_acc = 0;
-  if (p.dbg) t_start = clock64();
 
   // tile origin
   int n0 = 0, y0 = 0, x0 = 0;
@@ -359,7 +352,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
   else __syncthreads();
   pdl_trigger();        // the next kernel may start its prologue
   pdl_wait();           // A operand / residual come from predecessor kernels
-  if (p.dbg) t_setup = clock64();
 
   const int n_iters = kb1 - kb0;
   if (warp == PRODUCER_WARP) {
@@ -424,24 +416,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       e.x = x0 + r0 % p.bw;
       e.y = y0 + (r0 / p.bw) % p.bh;
       e.n = n0 + r0 / (p.bw * p.bh);
-    }
-    e.stats_base = -1;
-    if (p.stats) {
-      if (p.mode == 0) {
-        const int img = e.row0 / p.stats_rows_per_img, slot = (e.row0 % p.stats_rows_per_img) / 32;
-        if (e.row0 < p.M) e.stats_base = (static_cast<long long>(img) * p.stats_nslots + slot) * p.N;
-      } else if (e.x < p.W && e.y < p.H && e.n < p.NI) {
-        const int slot = (e.y / p.wbh) * p.stats_slots_x + e.x / p.wbw;
-        e.stats_base = (static_cast<long long>(e.n) * p.stats_nslots + slot) * p.N;
-      }
-    }
-    if (p.pf_bytes > 0) {
-      // one 128-byte line per prefetch; lines are spread over every epilogue thread of the grid
-      const long long nthr = static_cast<long long>(gridDim.x) * gridDim.y * gridDim.z * (32 * EW);
-      const long long me = ((static_cast<long long>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * (32 * EW) +
-                           threadIdx.x;
-      for (long long off = me * 128; off < p.pf_bytes; off += nthr * 128)
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p.pf_ptr + off));
     }
     // Per-column addends (bias + the row vector of this warp's image) of every chunk this warp will
     // finish, fetched now so that their L2 latency hides behind the mainloop: lane == column, one
@@ -518,7 +492,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
       wgmma_reg_fence(acc, BN / 2);
       if (prev >= 0) release(prev);
     }
-    if (p.dbg) t_acc = clock64();
     // every MMA of both warpgroups has retired -> the stage memory is free: accumulators -> blocks
     asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
     const uint32_t acc_base = smem_u32(smem);
@@ -539,6 +512,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     }
     asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
     e.res_base = acc_base + BN * BM * 4 + ew * (2 * EPI_TILE_BYTES);
+    // GroupNorm-statistics row of this warp, computed only now: the epilogue is its first reader, and the wide
+    // tiles sit at the 168-register limit, where a 64-bit value held across the mainloop makes ptxas spill
+    e.stats_base = -1;
+    if (p.stats) {
+      if (p.mode == 0) {
+        const int img = e.row0 / p.stats_rows_per_img, slot = (e.row0 % p.stats_rows_per_img) / 32;
+        if (e.row0 < p.M) e.stats_base = (static_cast<long long>(img) * p.stats_nslots + slot) * p.N;
+      } else if (e.x < p.W && e.y < p.H && e.n < p.NI) {
+        const int slot = (e.y / p.wbh) * p.stats_slots_x + e.x / p.wbw;
+        e.stats_base = (static_cast<long long>(e.n) * p.stats_nslots + slot) * p.N;
+      }
+    }
 
     constexpr int OUT_COLS = BN;            // accumulator columns that produce output (GEGLU: BN/2)
     const bool finalize = p.splits == 1;
@@ -664,10 +649,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
     }
     if (lane == 0) bulk_wait_read<0>();     // staging tiles must outlive the bulk stores' reads
     __syncwarp();
-    if (p.dbg && threadIdx.x == 0) {
-      long long* d = p.dbg + 8LL * ((static_cast<long long>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x);
-      d[0] = t_start; d[1] = t_setup; d[2] = t_acc; d[3] = clock64();
-    }
   }
   if constexpr (PAIR) cluster_sync_all();     // neither CTA may retire while the other can still signal it
 }
@@ -710,9 +691,8 @@ template <typename F>
 void for_each_plan(const PlanQuery& q, F f) {
   const int cands[5] = {256, 160, 128, 64, 32};
   const int sms = dbir_sm_count();
-  // CTA pairs (2-CTA clusters sharing B): DBIR_GEMM_PAIR = 0 never, 1 whenever the shape allows, unset: free choice
-  static const int pair_env = [] { const char* e = getenv("DBIR_GEMM_PAIR"); return e ? atoi(e) : -1; }();
-  const int pair_mode = q.pair_req == 1 ? 1 : q.pair_req == 2 ? 0 : pair_env;
+  // CTA pairs (2-CTA clusters sharing B): 0 never, 1 whenever the shape allows, -1 free choice
+  const int pair_mode = q.pair_req == 1 ? 1 : q.pair_req == 2 ? 0 : -1;
   const bool can_pair = pair_mode != 0 && !(q.m_tiles & 1);
   for (int i = 0; i < 10; ++i) {
     const int bn = cands[i % 5];
@@ -766,7 +746,6 @@ using PlanKey = std::array<long long, 20>;
 std::mutex g_plan_mu;                     // guards the cache
 std::mutex g_tune_mu;                     // serialises tuning (shared scratch / events, meaningful timings)
 std::map<PlanKey, TilePlan> g_plan_cache;
-int g_tuned_problems = 0;
 
 bool autotune_enabled() {
   static const int on = [] { const char* e = getenv("DBIR_GEMM_AUTOTUNE"); return e ? atoi(e) : 1; }();
@@ -819,8 +798,6 @@ bool tune_plan(const dbir_gemm_args* a, cudaStream_t st, const PlanQuery& q, Til
   if (!tune_reserve(&ts.out, &ts.out_cap, out_bytes)) return false;
   dbir_gemm_args t = *a;
   t.out = ts.out;
-  t.debug_stamps = nullptr;
-  t.prefetch_ptr = nullptr; t.prefetch_bytes = 0;
   if (a->gn_partials) {
     const long long imgs = a->a_mode == 1 ? a->img_n : a->M / a->gn_rows_per_img;
     const long long slots = a->a_mode == 1 ? dbir_gemm_gn_slots(a->img_h, a->img_w, 0)
@@ -877,7 +854,6 @@ TilePlan choose_plan(const dbir_gemm_args* a, cudaStream_t st, const PlanQuery& 
   if (tune_plan(a, st, q, &tuned)) plan = tuned;
   std::lock_guard<std::mutex> lk(g_plan_mu);
   g_plan_cache[key] = plan;
-  ++g_tuned_problems;
   return plan;
 }
 
@@ -895,12 +871,6 @@ extern "C" int dbir_gemm_model_plan(int32_t m_tiles, int32_t N, int32_t num_kb, 
   out[0] = t.bn; out[1] = t.splits; out[2] = t.kb_per_split; out[3] = t.pair;
   return 0;
 }
-/* Number of problem signatures tuned so far / drop every cached plan (tests, A/B runs). */
-extern "C" int32_t dbir_gemm_tuned_problems(void) { return g_tuned_problems; }
-extern "C" void dbir_gemm_clear_plans(void) {
-  std::lock_guard<std::mutex> lk(g_plan_mu);
-  g_plan_cache.clear();
-}
 
 namespace {
 int gemm_impl(const dbir_gemm_args* a, cudaStream_t st, const TilePlan* forced) {
@@ -909,7 +879,6 @@ int gemm_impl(const dbir_gemm_args* a, cudaStream_t st, const TilePlan* forced) 
                a->N, a->K);
   DBIR_REQUIRE(a->a && a->b && a->out, "dbir_gemm: null pointer");
   DBIR_REQUIRE(a->K % 8 == 0, "dbir_gemm: K=%d must be a multiple of 8 (16-byte rows)", a->K);
-  DBIR_REQUIRE(!a->out2, "dbir_gemm: out2 is not supported by the TMA-store epilogue");
   const int eb = a->out_kind == 0 ? 4 : 2;
   DBIR_REQUIRE((a->ldo * eb) % 16 == 0, "dbir_gemm: output row stride must be a multiple of 16 bytes (ldo=%lld)",
                (long long)a->ldo);
@@ -934,9 +903,6 @@ int gemm_impl(const dbir_gemm_args* a, cudaStream_t st, const TilePlan* forced) 
     else
       DBIR_REQUIRE(a->img_n % groups == 0, "dbir_gemm: grouped conv needs img_n %% groups == 0");
   }
-  p.dbg = reinterpret_cast<long long*>(a->debug_stamps);
-  p.pf_ptr = reinterpret_cast<const char*>(a->prefetch_ptr);
-  p.pf_bytes = a->prefetch_ptr ? a->prefetch_bytes : 0;
   if (a->geglu)
     DBIR_REQUIRE(a->force_bn >= 64 && a->force_bn != 160 && a->N % a->force_bn == 0 && !a->residual,
                  "dbir_gemm: GEGLU needs force_bn in {64,128,256} dividing N (weights are packed per tile)");

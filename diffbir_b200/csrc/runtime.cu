@@ -5,7 +5,6 @@
 #include <cudaTypedefs.h>
 #include <stdarg.h>
 #include <string.h>
-#include <stdlib.h>
 
 static thread_local char g_err[1024] = "";
 
@@ -18,13 +17,9 @@ void dbir_set_error(const char* fmt, ...) {
 
 extern "C" const char* dbir_last_error(void) { return g_err; }
 extern "C" const char* dbir_version(void) {
-  return "diffbir_b200 0.1 (sm_90a; wgmma/TMA)";
+  return "diffbir_b200 0.2 (sm_90a; wgmma/TMA)";
 }
 extern "C" int dbir_operand_kind(void) { return DBIR_OPERAND_KIND; }
-extern "C" int dbir_pdl_enabled(void) {
-  static const int on = [] { const char* e = getenv("DBIR_PDL"); return e ? atoi(e) : 1; }();
-  return on;
-}
 
 extern "C" int dbir_sm_count(void) {
   static int sms = 0;

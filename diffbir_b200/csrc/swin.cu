@@ -148,10 +148,3 @@ extern "C" int dbir_window_attention(const void* qkv, int64_t ldq, int32_t batch
   dbir_set_error("dbir_window_attention: unsupported heads x head_dim %d x %d", heads, head_dim);
   return -2;
 }
-
-extern "C" int dbir_swin_window_attention(const void* qkv, int64_t ldq, int32_t batch, int32_t h,
-                                          int32_t w, int32_t heads, int32_t head_dim,
-                                          int32_t window, int32_t shift, const float* bias_table,
-                                          void* out, int64_t ldo, void* stream) {
-  return dbir_window_attention(qkv, ldq, batch, h, w, heads, head_dim, window, shift, bias_table, -100.0f, out, ldo, stream);
-}

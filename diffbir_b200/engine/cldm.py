@@ -155,7 +155,6 @@ class CldmEngine:
                     cat = torch.cat([wu, wc], 0).contiguous()
                     self.twin_w[k] = cat
                     self.unet.w[k], self.cnet.w[k] = cat[: wu.shape[0]], cat[wu.shape[0]:]
-        self.group_twins = os.environ.get("DBIR_GROUP_TWINS", "1") != "0"
         self.ws = Workspace(self.dev)
         self.op_dtype = lib.operand_dtype()
         self.kv: Dict[str, torch.Tensor] = {}      # per attention layer: op16 [nb*77, 2C]
@@ -167,9 +166,6 @@ class CldmEngine:
         self._side = None
         self._ts_key = None
         self._part = {}                  # fp32 activation data_ptr -> (GN partial-sum buffer, slots)
-        self._wseq, self._wpos = {}, {}  # per-stream weight sequence of the forward (L2 prefetch lookahead)
-        self.prefetch_weights = False    # opt-in: L2 prefetch of the next layers' weights during a GEMM
-        self.fuse_gn_stats = True
         # Batch-invariant kernel plans: no split-K, whole attention tiles per CTA. Every sample's result
         # then has the same bits whatever batch it runs in (tiled sampling: sharded == single rank) and
         # whatever plan the timing-based tuner picked (run-to-run / process-to-process reproducible).
@@ -257,26 +253,11 @@ class CldmEngine:
         self.emb_cur.copy_(self.emb_table[step_idx])
 
     def _gemm(self, tag: str, a, b, *args, **kw):
-        """dbir_gemm with this stream's split-K scratch (64 MiB, zero-initialised once) and an L2
-        prefetch of the weights of the GEMM that follows on the same stream (weights are the only
-        cold operand of a forward: 2.5 GB streamed from HBM per step, activations are L2-resident).
-        The weight sequence is learnt on the previous forward (it never changes)."""
+        """dbir_gemm with this stream's split-K scratch (64 MiB, zero-initialised once)."""
         ws = self.ws.get(tag + ":splitk", (16 * 1024 * 1024 + 16384,), torch.float32, zero=True)
-        seq = self._wseq.setdefault(tag, [])
-        i = self._wpos.get(tag, 0)
-        wbytes = b.numel() * b.element_size()
-        if i < len(seq):
-            if seq[i][0] != b.data_ptr():          # sequence changed (other shapes): relearn
-                del seq[i:]
-        if i >= len(seq):
-            seq.append((b.data_ptr(), wbytes))
-        self._wpos[tag] = i + 1
-        pf = None
-        if self.prefetch_weights and i + 1 < len(seq):
-            pf = seq[i + 1]
         if self.batch_invariant:
             kw.setdefault("split_k", 1)
-        lib.gemm(a, b, *args, splitk_ws=ws, prefetch=pf, **kw)
+        lib.gemm(a, b, *args, splitk_ws=ws, **kw)
 
     def _emb(self, tag: str, l: arch.Layer, nb: int) -> torch.Tensor:
         """Time-embedding rows of ResBlock l for this call's images; tag "g" = both twins ([UNet ; ControlNet])."""
@@ -300,7 +281,7 @@ class CldmEngine:
         stats = ws.get(tag + ":gn_stats", (nb * 64,), torch.float32)
         p1 = self._part.get(src1.data_ptr())
         p2 = self._part.get(src2.data_ptr()) if src2 is not None else None
-        if self.fuse_gn_stats and p1 is not None and (src2 is None or p2 is not None):
+        if p1 is not None and (src2 is None or p2 is not None):
             lib.gn_finalize(p1[0], p1[1], c1, p2[0] if p2 else None, p2[1] if p2 else 0, c2, nb, h * w, eps, stats)
         else:
             wsp = ws.get(tag + ":gn_ws", (lib.gn_workspace_floats(nb, h * w, c1 + c2),), torch.float32, zero=True)
@@ -310,8 +291,6 @@ class CldmEngine:
 
     def _stats_kw(self, out: torch.Tensor, nb: int, n_cols: int, conv_hw=None, rows_per_img: int = 0) -> dict:
         """kwargs that make dbir_gemm emit GroupNorm partial sums for its output tensor `out`."""
-        if not self.fuse_gn_stats:
-            return {}
         slots = lib.gemm_gn_slots(*conv_hw) if conv_hw else lib.gemm_gn_slots(0, 0, rows_per_img)
         if slots <= 0:
             self._part.pop(out.data_ptr(), None)
@@ -434,8 +413,8 @@ class CldmEngine:
         """Grouped twin launches need every stacked problem to start on a 128-row tile boundary (plain
         GEMMs) and conv tiles not to straddle the two nets: true for even nb with >= 64 pixels at the
         coarsest level (the 512^2 / tiled production shapes); reduced test shapes take the two-stream path."""
-        if not self.group_twins or set(l.prefix for blk in self.cnet.plan.input_blocks[1:] + [self.cnet.plan.middle]
-                                       for l in blk.layers) - self.twin_prefixes:
+        if set(l.prefix for blk in self.cnet.plan.input_blocks[1:] + [self.cnet.plan.middle]
+               for l in blk.layers) - self.twin_prefixes:
             return False
         ch, cw = h, w
         for blk in self.unet.plan.input_blocks:
@@ -498,8 +477,7 @@ class CldmEngine:
         """Returns (graph, x_in, c_img, eps, kernels_per_replay): static input/output buffers and
         a CUDA graph of forward(x_in, c_img) -> eps, captured once per (shape, strength) and
         reused across images (set_context / load_step only rewrite buffers the graph reads)."""
-        key = (nb, c, h, w, tuple(float(s) for s in control_scales), self.two_streams, self.batch_invariant,
-               self.group_twins)
+        key = (nb, c, h, w, tuple(float(s) for s in control_scales), self.two_streams, self.batch_invariant)
         hit = self._graphs.get(key)
         if hit is not None:
             return hit
@@ -533,7 +511,6 @@ class CldmEngine:
         assert c_img.is_cuda and c_img.dtype == torch.float32 and c_img.is_contiguous()
         nb, _, h, w = x.shape
         assert nb == self._nb == self.emb_nb, "set_context / set_timesteps batch mismatch"
-        self._wpos = {}
         ws, U, Cn = self.ws, self.unet, self.cnet
         # 1+2. UNet encoder + middle and the ControlNet. Production shapes: their twin layers run as ONE
         #      stream of grouped launches on batch-stacked activations (_encoder_twins). Otherwise: UNet

@@ -1,8 +1,6 @@
 """Shared engine plumbing: named workspace buffers and weight packing helpers."""
 from __future__ import annotations
 
-import os
-
 from typing import Dict, Tuple
 
 import torch
@@ -34,9 +32,6 @@ class Workspace:
             self._bufs[key] = buf
         return buf[:n].view(*shape)
 
-    def bytes(self) -> int:
-        return sum(b.numel() * b.element_size() for b in self._bufs.values())
-
 
 class GraphCache:
     """CUDA graphs of a fixed-shape function of device tensors, one per key (input shapes).
@@ -48,7 +43,6 @@ class GraphCache:
 
     def __init__(self, ws: "Workspace" = None):
         self._g = {}
-        self.enabled = True
         if ws is not None:
             ws.on_grow = self._g.clear
 
@@ -56,7 +50,7 @@ class GraphCache:
         self._g.clear()
 
     def run(self, key, fn, *inputs: torch.Tensor):
-        if not self.enabled or torch.cuda.is_current_stream_capturing():
+        if torch.cuda.is_current_stream_capturing():
             return fn(*inputs)
         hit = self._g.get(key)
         if hit is None:
@@ -109,9 +103,8 @@ def geglu_tile(c: int) -> int:
     """GEMM tile width used for the GEGLU projection of a width-c transformer block (the weights are packed
     per tile as [values | gates], so it is fixed at load time)."""
     # 256-wide tiles (128 values + 128 gates): at large batch the projection is bound by L2 -> SM operand
-    # traffic, which a 256-wide tile (and a CTA pair sharing it) cuts against 128-wide ones. DBIR_GEGLU_TILE overrides.
-    forced = int(os.environ.get("DBIR_GEGLU_TILE", "0"))       # A/B switch: 64 | 128 | 256
-    for bn in ((forced,) if forced else ()) + (256, 128, 64):
+    # traffic, which a 256-wide tile (and a CTA pair sharing it) cuts against 128-wide ones.
+    for bn in (256, 128, 64):
         if (8 * c) % bn == 0:
             return bn
     return 64

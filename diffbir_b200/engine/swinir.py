@@ -129,7 +129,7 @@ class SwinIREngine:
                 shift = 0 if bi % 2 == 0 else 4
                 lib.layernorm(t, cp, M, c, W[p + "norm1.weight"], W[p + "norm1.bias"], ln16, cp)
                 lib.gemm(ln16, W[p + "qkv.w"], qkv, M=M, N=3 * c, K=cp, bias=W[p + "qkv.b"], ldo=self.qkv_ld)
-                lib.swin_window_attention(qkv, self.qkv_ld, nb, h, w, shift, W[p + "rpb"], att, cp)
+                lib.window_attention(qkv, self.qkv_ld, nb, h, w, 6, 30, shift, W[p + "rpb"], -100.0, att, cp)
                 lib.gemm(att, W[p + "proj.w"], t, M=M, N=c, K=cp, bias=W[p + "proj.b"], residual=t,
                          ldo=cp, ldr=cp)
                 lib.layernorm(t, cp, M, c, W[p + "norm2.weight"], W[p + "norm2.bias"], ln16, cp)

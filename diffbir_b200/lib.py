@@ -18,8 +18,6 @@ _OPERANDS = os.environ.get("DBIR_OPERANDS", "fp16").lower()
 if _OPERANDS not in ("fp16", "bf16"):
     raise ValueError(f"DBIR_OPERANDS={_OPERANDS!r}: expected fp16 or bf16")
 LIB_PATH = _HERE / ("libdiffbir_b200_bf16.so" if _OPERANDS == "bf16" else "libdiffbir_b200.so")
-if os.environ.get("DBIR_LIB_TAG"):      # experiment builds: python -m diffbir_b200.build --tag=<tag> -D...
-    LIB_PATH = _HERE / f"libdiffbir_b200_{os.environ['DBIR_LIB_TAG']}.so"
 _lib = None
 _launches = 0  # kernels launched through this binding (bench.py reports it)
 
@@ -41,12 +39,9 @@ class GemmArgs(C.Structure):
         ("geglu", C.c_int32), ("force_bn", C.c_int32),
         ("alpha", C.c_float), ("act_param", C.c_float),
         ("bias_per_row", C.c_int32), ("groups", C.c_int32),
-        ("out2", C.c_void_p), ("ldo2", C.c_int64),
         ("splitk_ws", C.c_void_p), ("splitk_ws_bytes", C.c_int64),
         ("split_k", C.c_int32), ("cta_pair", C.c_int32),
-        ("debug_stamps", C.c_void_p),
-        ("gn_partials", C.c_void_p), ("gn_rows_per_img", C.c_int32), ("reserved2", C.c_int32),
-        ("prefetch_ptr", C.c_void_p), ("prefetch_bytes", C.c_int64),
+        ("gn_partials", C.c_void_p), ("gn_rows_per_img", C.c_int32),
     ]
 
 
@@ -72,23 +67,6 @@ def check(rc: int, what: str = ""):
         raise DbirError(f"{what} failed (rc={rc}): {msg}")
 
 
-_profile = None   # list of (kind, flops, start_event, end_event) while profiling
-
-
-def profile_begin():
-    """bench.py's kernel census: brackets every GEMM / attention launch with CUDA events."""
-    global _profile
-    _profile = []
-
-
-def profile_end():
-    global _profile
-    torch.cuda.synchronize()
-    out = [(k, info, fl, e0.elapsed_time(e1)) for k, info, fl, e0, e1 in _profile]
-    _profile = None
-    return out
-
-
 _record = None    # list of (kind, info, flops, thunk) while recording
 
 
@@ -103,23 +81,6 @@ def record_end():
     global _record
     out, _record = _record, None
     return out
-
-
-class _Prof:
-    def __init__(self, kind, info, flops):
-        self.kind, self.info, self.flops = kind, info, flops
-
-    def __enter__(self):
-        if _profile is not None:
-            self.e0 = torch.cuda.Event(enable_timing=True)
-            self.e1 = torch.cuda.Event(enable_timing=True)
-            self.e0.record()
-        return self
-
-    def __exit__(self, *a):
-        if _profile is not None:
-            self.e1.record()
-            _profile.append((self.kind, self.info, self.flops, self.e0, self.e1))
 
 
 def count_launch(n: int = 1):
@@ -148,8 +109,8 @@ ACT = {None: 0, "none": 0, "gelu": 1, "lrelu": 2, "silu": 3}
 
 def gemm(a, b, out, *, M, N, K, bias=None, rowvec=None, rows_per_vec=0, residual=None,
          lda=0, ldb=0, ldo=None, ldr=None, conv=None, act=None, act_param=0.0, alpha=1.0,
-         geglu=False, force_bn=0, bias_per_row=False, out2=None, ldo2=None, splitk_ws=None,
-         split_k=0, cta_pair=0, debug_stamps=None, gn_partials=None, gn_rows_per_img=0, prefetch=None, groups=1):
+         geglu=False, force_bn=0, bias_per_row=False, splitk_ws=None, split_k=0, cta_pair=0,
+         gn_partials=None, gn_rows_per_img=0, groups=1):
     """out = residual + alpha * act(A @ B^T + bias + rowvec). conv = (n, h, w, c, ksize)."""
     lib = load()
     g = GemmArgs()
@@ -174,20 +135,14 @@ def gemm(a, b, out, *, M, N, K, bias=None, rowvec=None, rows_per_vec=0, residual
     g.force_bn = force_bn
     g.bias_per_row = 1 if bias_per_row else 0
     g.groups = groups
-    g.out2 = _ptr(out2)
-    g.ldo2 = (n_out if ldo2 is None else ldo2)
     if splitk_ws is not None:
         g.splitk_ws = splitk_ws.data_ptr()
         g.splitk_ws_bytes = splitk_ws.numel() * splitk_ws.element_size()
     g.split_k = split_k
     g.cta_pair = cta_pair
-    g.debug_stamps = _ptr(debug_stamps)
     g.gn_partials = _ptr(gn_partials)
     g.gn_rows_per_img = gn_rows_per_img
-    if prefetch is not None:
-        g.prefetch_ptr, g.prefetch_bytes = prefetch
-    with _Prof("conv" if conv is not None else "gemm", (M, N, K), 2.0 * M * N * K):
-        check(lib.dbir_gemm(C.byref(g), C.c_void_p(stream_ptr())), "dbir_gemm")
+    check(lib.dbir_gemm(C.byref(g), C.c_void_p(stream_ptr())), "dbir_gemm")
     if _record is not None:
         keep = (a, b, out, bias, rowvec, residual, splitk_ws, gn_partials)     # keep buffers alive
         _record.append(("conv" if conv is not None else "gemm", (M, N, K), 2.0 * M * N * K,
@@ -204,7 +159,7 @@ def _fp(t):
 
 
 def attention_ws_bytes(batch, heads, sq, skv) -> int:
-    """Bytes of (zero-initialised, per-stream) workspace that let dbir_attention_sk balance this
+    """Bytes of (zero-initialised, per-stream) workspace that let dbir_attention balance this
     shape over all SMs; 0 when whole tiles per CTA are used anyway."""
     lib = load()
     lib.dbir_attention_ws_bytes.restype = C.c_int64
@@ -217,11 +172,10 @@ def attention(q, k, v, out, *, batch, heads, sq, skv, ldq, ldk, ldv, ldo, ws=Non
     ws_bytes = ws.numel() * ws.element_size() if ws is not None else 0
 
     def call():
-        check(load().dbir_attention_sk(_fp(q), _fp(k), _fp(v), _fp(out), batch, heads, sq, skv,
-                                       C.c_int64(ldq), C.c_int64(ldk), C.c_int64(ldv), C.c_int64(ldo),
-                                       _fp(ws), C.c_int64(ws_bytes), _sp()), "dbir_attention_sk")
-    with _Prof("attention", (batch, heads, sq, skv), 4.0 * batch * heads * sq * skv * 64):
-        call()
+        check(load().dbir_attention(_fp(q), _fp(k), _fp(v), _fp(out), batch, heads, sq, skv,
+                                    C.c_int64(ldq), C.c_int64(ldk), C.c_int64(ldv), C.c_int64(ldo),
+                                    _fp(ws), C.c_int64(ws_bytes), _sp()), "dbir_attention")
+    call()
     if _record is not None:
         _record.append(("attention", (batch, heads, sq, skv), 4.0 * batch * heads * sq * skv * 64, call))
     count_launch()
@@ -231,15 +185,6 @@ def gn_workspace_floats(n, hw, c) -> int:
     lib = load()
     lib.dbir_gn_workspace_floats.restype = C.c_int64
     return int(lib.dbir_gn_workspace_floats(n, hw, c))
-
-
-def gemm_tuned_problems() -> int:
-    """Problem signatures dbir_gemm has planned (autotuned) so far."""
-    return int(load().dbir_gemm_tuned_problems())
-
-
-def gemm_clear_plans() -> None:
-    load().dbir_gemm_clear_plans()
 
 
 def gemm_gn_slots(conv_h=0, conv_w=0, rows_per_img=0) -> int:
@@ -276,13 +221,6 @@ def layernorm(x, ldx, rows, c, gamma, beta, out, ldo, eps=1e-5, rows_per_group=0
 def window_attention(qkv, ldq, batch, h, w, heads, head_dim, shift, bias_table, mask_value, out, ldo):
     check(load().dbir_window_attention(_fp(qkv), C.c_int64(ldq), batch, h, w, heads, head_dim, 8, shift, _fp(bias_table),
                                        C.c_float(mask_value), _fp(out), C.c_int64(ldo), _sp()), "dbir_window_attention")
-    count_launch()
-
-
-def swin_window_attention(qkv, ldq, batch, h, w, shift, bias_table, out, ldo):
-    check(load().dbir_swin_window_attention(_fp(qkv), C.c_int64(ldq), batch, h, w, 6, 30, 8, shift,
-                                            _fp(bias_table), _fp(out), C.c_int64(ldo), _sp()),
-          "dbir_swin_window_attention")
     count_launch()
 
 

@@ -58,20 +58,14 @@ typedef struct dbir_gemm_args {
                            ControlNet encoders' twin layers): A / out / residual / rowvec / gn_partials hold the G
                            problems back to back along M (M = total rows, divisible by G; conv: img_n divisible by
                            G), b is [G*N, ldb] and bias [G*N] (group g's weights at rows g*N). */
-  void* out2;           /* optional op16 copy of the result [rows, ldo2] (operand of the next op) */
-  int64_t ldo2;
   void* splitk_ws;      /* optional split-K scratch (zero-initialised once by the caller, >= 64 KiB +
                            partial tiles); NULL disables split-K. Summation order is fixed. */
   int64_t splitk_ws_bytes;
   int32_t split_k;      /* 0 = auto, 1 = off, n > 1 = force n splits */
   int32_t cta_pair;     /* CTA pairs (2-CTA clusters sharing the B tile by TMA multicast): 0 = auto, 1 = whenever the tile count is even, 2 = never */
-  void* debug_stamps;   /* optional int64 [ctas][8] clock64 stamps (start, setup, acc ready, end) */
   void* gn_partials;    /* optional fp32 [img][dbir_gemm_gn_slots()][N][2]: per 32-row-slot column sums and
                            sums of squares of the OUTPUT (fused GroupNorm statistics; see dbir_gn_finalize) */
   int32_t gn_rows_per_img; /* matrix mode only: rows per image (multiple of 32); conv mode uses img_h*img_w */
-  int32_t reserved2;
-  const void* prefetch_ptr; /* optional: memory a later kernel will stream (next layers' weights); pulled into */
-  int64_t prefetch_bytes;   /* L2 by the idle epilogue warps during this kernel's mainloop */
 } dbir_gemm_args;
 /* Number of 32-row slots per image dbir_gemm writes into gn_partials (conv: h, w > 0; matrix: rows_per_img). */
 int32_t dbir_gemm_gn_slots(int32_t conv_h, int32_t conv_w, int32_t rows_per_img);
@@ -80,11 +74,9 @@ int dbir_gemm(const dbir_gemm_args* args, void* stream);
  * for a signature made outside stream capture times the candidate plans on the caller's operands
  * (outputs redirected to scratch, cold L2) and caches the fastest; DBIR_GEMM_AUTOTUNE=0 selects
  * the analytic model instead (bit-reproducible across processes: split-K changes summation order). */
-int32_t dbir_gemm_tuned_problems(void);   /* signatures planned so far */
 /* the analytic model's plan for a tile grid, host only: out[0..3] = BN, splits, k-blocks per split, pair */
 int dbir_gemm_model_plan(int32_t m_tiles, int32_t N, int32_t num_kb, int32_t geglu, int32_t force_bn,
                          int32_t split_k, int32_t cta_pair, int64_t ws_floats, int32_t* out);
-void dbir_gemm_clear_plans(void);         /* forget every cached plan */
 
 /* ---- flash attention, head_dim 64 (wgmma) --------------------------------------------
  * out[b, i, h*64 + :] = softmax_j(q_h[i] . k_h[j] / 8) v_h[j]; q/k/v/out are op16 matrices
@@ -92,17 +84,14 @@ void dbir_gemm_clear_plans(void);         /* forget every cached plan */
  * Replaces F.scaled_dot_product_attention and the head split/merge copies in
  * SDPCrossAttention.forward (attention.py:189-216); kv = text context for attn2.
  */
+/* The optional workspace enables the stream-K decomposition: when whole 128-query tiles would
+ * leave the last wave of CTA slots (two per SM) mostly idle, every CTA instead takes an equal share
+ * of the (tile, 64-key step) space and tiles cut by a CTA boundary are combined through `ws` (fixed
+ * part order: deterministic). ws: dbir_attention_ws_bytes() bytes, zero-initialised once by the
+ * caller, private to one stream; NULL / too small = whole tiles per CTA. */
 int dbir_attention(const void* q, const void* k, const void* v, void* out, int32_t batch,
                    int32_t heads, int32_t sq, int32_t skv, int64_t ldq, int64_t ldk, int64_t ldv,
-                   int64_t ldo, void* stream);
-/* Same, with an optional workspace that enables the stream-K decomposition: when whole 128-query
- * tiles would leave the last wave of CTA slots (two per SM) mostly idle, every CTA instead takes an
- * equal share of the (tile, 64-key step) space and tiles cut by a CTA boundary are combined through
- * `ws` (fixed part order: deterministic). ws: dbir_attention_ws_bytes() bytes, zero-initialised once
- * by the caller, private to one stream; NULL / too small = whole tiles per CTA. */
-int dbir_attention_sk(const void* q, const void* k, const void* v, void* out, int32_t batch,
-                      int32_t heads, int32_t sq, int32_t skv, int64_t ldq, int64_t ldk,
-                      int64_t ldv, int64_t ldo, void* ws, int64_t ws_bytes, void* stream);
+                   int64_t ldo, void* ws, int64_t ws_bytes, void* stream);
 int64_t dbir_attention_ws_bytes(int32_t batch, int32_t heads, int32_t sq, int32_t skv);  /* 0: not needed */
 
 /* ---- GroupNorm (32 groups) / LayerNorm ------------------------------------------------
@@ -136,19 +125,16 @@ int dbir_layernorm(const float* x, int64_t ldx, int32_t rows, int32_t c, const f
 /* imgs_per_group / rows_per_group > 0: stacked twin problems (see dbir_gemm_args.groups) -- image n /
  * row r takes gamma / beta at offset (n / imgs_per_group) * C resp. (r / rows_per_group) * c. 0 = one set. */
 
-/* ---- SwinIR window attention -----------------------------------------------------------
+/* ---- SwinIR / SCUNet window attention --------------------------------------------------
  * One 8x8 window per CTA; qkv op16 [batch*h*w, ldq] with columns [q | k | v] x (heads, dim)
  * as produced by WindowAttention.qkv (swinir.py:104,122-123); out op16 [batch*h*w, ldo]
  * (first heads*dim columns) in original token order. shift = 0 (W-MSA) or 4 (SW-MSA):
  * replaces torch.roll + window_partition + q k^T + bias + mask + softmax + @v +
  * window_reverse + roll (swinir.py:120-151, 255-276).
+ * (heads, head_dim) = 6 x 30 (SwinIR) or {1,2,4,8} x 32 (SCUNet's WMSA, scunet.py:9-99: same roll / window /
+ * relative-position-bias / region-mask structure); mask_value is added to the logits of token pairs from
+ * different shift regions (-100 in SwinIR, -inf in SCUNet).
  */
-int dbir_swin_window_attention(const void* qkv, int64_t ldq, int32_t batch, int32_t h, int32_t w,
-                               int32_t heads, int32_t head_dim, int32_t window, int32_t shift,
-                               const float* bias_table, void* out, int64_t ldo, void* stream);
-/* Same kernel for other (heads, head_dim) pairs -- 6 x 30 (SwinIR) and {1,2,4,8} x 32 (SCUNet's WMSA, scunet.py:9-99:
- * same roll / window / relative-position-bias / region-mask structure) -- and an explicit mask value added to the
- * logits of token pairs from different shift regions (-100 in SwinIR, -inf in SCUNet). */
 int dbir_window_attention(const void* qkv, int64_t ldq, int32_t batch, int32_t h, int32_t w, int32_t heads,
                           int32_t head_dim, int32_t window, int32_t shift, const float* bias_table, float mask_value,
                           void* out, int64_t ldo, void* stream);

@@ -398,9 +398,10 @@ def test_fused_groupnorm_statistics(L, n, h, w, c1, c2):
 
 
 @pytest.mark.parametrize("b,h,w,shift", [(1, 64, 64, 0), (1, 64, 64, 4), (2, 16, 24, 4), (1, 128, 64, 4)])
-def test_swin_window_attention(L, b, h, w, shift):
-    """dbir_swin_window_attention stand-alone (WindowAttention.forward + roll / partition / reverse /
-    shift mask, swinir.py:120-151, 245-285) vs the oracle's op sequence in fp32 on the same 16-bit qkv."""
+def test_window_attention_swinir(L, b, h, w, shift):
+    """dbir_window_attention with SwinIR's 6 heads x 30 and shift mask -100, stand-alone (WindowAttention.forward
+    + roll / partition / reverse / shift mask, swinir.py:120-151, 245-285) vs the oracle's op sequence in fp32 on
+    the same 16-bit qkv."""
     from oracle.swinir import rel_pos_index, shift_mask
     heads, dh, ws = 6, 30, 8
     c = heads * dh
@@ -411,7 +412,7 @@ def test_swin_window_attention(L, b, h, w, shift):
     qkv[:, :3 * c] = (torch.randn(b * h * w, 3 * c, generator=g) * 1.5).to("cuda", dt)
     table = (torch.randn(225, heads, generator=g) * 0.5).cuda()
     out = torch.zeros(b * h * w, 192, dtype=dt, device="cuda")
-    lib.swin_window_attention(qkv, ld, b, h, w, shift, table, out, 192)
+    lib.window_attention(qkv, ld, b, h, w, heads, dh, shift, table, -100.0, out, 192)
     # reference (fp32, on the fp16/bf16-rounded qkv)
     y = qkv[:, :3 * c].float().view(b, h, w, 3 * c)
     if shift:

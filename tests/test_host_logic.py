@@ -164,7 +164,6 @@ def test_c_abi_exports_every_declared_symbol():
         build_library()
     lib = ctypes.CDLL(str(so))
     header = (ROOT / "include" / "diffbir_b200.h").read_text()
-    header = re.sub(r"#ifdef DBIR_DEBUG_PROBES.*?#endif", "", header, flags=re.S)      # probe builds only
     names = sorted(set(re.findall(r"\b(dbir_[a-z0-9_]+)\s*\(", header)) - {"dbir_gemm_args"})
     assert not hasattr(lib, "dbir_debug_mma_rate"), "calibration probes must not ship in the product library"
     assert len(names) >= 20
