@@ -17,6 +17,12 @@ namespace {
 
 constexpr int GN_THREADS = 256;
 constexpr int GN_WARPS = GN_THREADS / 32;
+// gn_stats workspace: one fixed-size region per image, [ticket (padded to 64 floats) | partials[<= 1024 chunks][32][2]].
+// The offsets do not depend on the batch size, so calls with different batches can share one workspace: the
+// tickets of image n never lie under another call's partial sums. (A layout of all tickets first and the partials
+// after them moved the partials with the batch: a small batch wrote partial sums over the tickets a later, larger
+// batch counted on, and those images kept stale statistics.)
+constexpr long long GN_IMG_FLOATS = 64 + 1024LL * 64;
 
 __device__ __forceinline__ const float* cat_ptr(const float* s1, const float* s2, int c1, int c2,
                                                 long long pix, int c) {
@@ -27,13 +33,12 @@ __device__ __forceinline__ const float* cat_ptr(const float* s1, const float* s2
 // Stage 1: per-group sum / sum of squares over a chunk of pixels.
 // grid = (chunks, N). A warp sweeps 128-channel slabs (one float4 per lane, coalesced) over the
 // chunk's pixels keeping per-lane register sums, folds them into 32 per-group shared-memory
-// accumulators, and the CTA writes 64 floats: partial[N][chunks][32][2].
+// accumulators, and the CTA writes 64 floats into its image's workspace region: partials[chunk][32][2].
 // The last CTA of each image (atomic ticket, self-resetting) combines the chunk partials in fp64
 // in a fixed order -> deterministic mean / rstd.
 __global__ void __launch_bounds__(GN_THREADS)
 gn_stats_kernel(const float* __restrict__ s1, const float* __restrict__ s2, int c1, int c2,
-                int hw, int pix_per_chunk, float* __restrict__ partial,
-                unsigned int* __restrict__ tickets, float* __restrict__ stats, float eps) {
+                int hw, int pix_per_chunk, float* __restrict__ workspace, float* __restrict__ stats, float eps) {
   pdl_trigger();
   pdl_wait();
   const int C = c1 + c2;
@@ -91,7 +96,10 @@ gn_stats_kernel(const float* __restrict__ s1, const float* __restrict__ s2, int 
     __syncwarp();
   }
   __syncthreads();
-  float* my_partial = partial + (static_cast<long long>(n) * chunks + chunk) * 64;
+  float* img_ws = workspace + static_cast<long long>(n) * GN_IMG_FLOATS;
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(img_ws);
+  float* img_partial = img_ws + 64;
+  float* my_partial = img_partial + chunk * 64;
   if (threadIdx.x < 64) {
     float a = 0.f;
 #pragma unroll
@@ -103,14 +111,13 @@ gn_stats_kernel(const float* __restrict__ s1, const float* __restrict__ s2, int 
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
-    const unsigned int t = atomicAdd(&tickets[n], 1u);
+    const unsigned int t = atomicAdd(ticket, 1u);
     s_last = (t == static_cast<unsigned int>(chunks) - 1);
-    if (s_last) tickets[n] = 0;   // self-reset for the next launch
+    if (s_last) *ticket = 0;      // self-reset for the next launch
   }
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  const float* img_partial = partial + static_cast<long long>(n) * chunks * 64;
   for (int g = warp; g < 32; g += GN_WARPS) {
     double a = 0.0, b = 0.0;
     for (int ch = lane; ch < chunks; ch += 32) {
@@ -372,9 +379,9 @@ layernorm_kernel(const float* __restrict__ x, long long ldx, int rows, int C,
 }  // namespace
 
 extern "C" int64_t dbir_gn_workspace_floats(int32_t n, int32_t hw, int32_t c) {
-  // tickets + partials [n][chunks <= 1024][32][2]
+  // per image: ticket + partials [chunks <= 1024][32][2] (GN_IMG_FLOATS)
   (void)hw; (void)c;
-  return 64 + ((static_cast<int64_t>(n) + 3) / 4) * 4 + static_cast<int64_t>(n) * 1024 * 64 + 64;
+  return static_cast<int64_t>(n) * GN_IMG_FLOATS;
 }
 
 static int gn_chunks(int n, int hw, int* pix_per_chunk) {
@@ -399,11 +406,8 @@ extern "C" int dbir_gn_stats(const float* src1, const float* src2, int32_t c1, i
   DBIR_REQUIRE(c2 == 0 || src2, "dbir_gn_stats: src2 missing");
   int ppc;
   const int chunks = gn_chunks(n, hw, &ppc);
-  unsigned int* tickets = reinterpret_cast<unsigned int*>(workspace);
-  float* partial = workspace + 64 + ((n + 3) / 4) * 4;
   DBIR_CHECK_CUDA(dbir_launch(gn_stats_kernel, dim3(chunks, n), dim3(GN_THREADS), 0,
-                              reinterpret_cast<cudaStream_t>(stream), src1, src2, c1, c2, hw, ppc, partial, tickets,
-                              stats, eps));
+                              reinterpret_cast<cudaStream_t>(stream), src1, src2, c1, c2, hw, ppc, workspace, stats, eps));
   return 0;
 }
 

@@ -248,6 +248,17 @@ class CldmEngine:
         self.timesteps = list(timesteps)
         self._ts_key = key
 
+    def release_buffers(self) -> None:
+        """Frees everything sized by the batch of the last forward: captured graphs, workspace, cross-attention
+        K/V and the time-embedding table. Packed weights stay; the next set_context / set_timesteps / forward
+        re-create the rest."""
+        self.ws.clear()                     # also drops the graphs (on_grow)
+        self._part.clear()
+        self.kv.clear()
+        self.emb_table = self.emb_cur = None
+        self._ts_key = None
+        self._nb = self.emb_nb = 0
+
     def load_step(self, step_idx: int):
         """Selects the time embedding of sampler step `step_idx` (one D2D copy, outside graphs)."""
         self.emb_cur.copy_(self.emb_table[step_idx])

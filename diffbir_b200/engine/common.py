@@ -32,6 +32,12 @@ class Workspace:
             self._bufs[key] = buf
         return buf[:n].view(*shape)
 
+    def clear(self) -> None:
+        """Drops every buffer (graphs that hold their pointers must be dropped with them)."""
+        if self.on_grow is not None:
+            self.on_grow()
+        self._bufs.clear()
+
 
 class GraphCache:
     """CUDA graphs of a fixed-shape function of device tensors, one per key (input shapes).

@@ -104,6 +104,17 @@ class VaeEngine:
         lib.gemm(b16, W[p + "conv2.weight"], out, M=M, N=cout, K=9 * cout, bias=W[p + "conv2.bias"],
                  residual=res, conv=(nb, h, w, cout, 3), **self._stats_kw(out, nb, cout, h, w))
 
+    def release_buffers(self) -> None:
+        """Frees the workspace and the captured encode / decode graphs; the next call re-creates them."""
+        self.ws.clear()                          # also drops the graphs (GraphCache hooks on_grow)
+        self._part.clear()
+
+    @staticmethod
+    def attn_rows(hw: int) -> int:
+        """Query rows per chunk of the mid attention's materialised S: 8192 up to 65536 tokens (2048^2 images),
+        beyond that a multiple of 128 that keeps the fp32 S at or below 2 GiB (3584 rows at 3072^2)."""
+        return min(8192, max(128, (2 ** 31 // (4 * hw)) // 128 * 128))
+
     def _attn(self, p, x, c, nb, h, w):
         """Single-head attention over pixels, in place on x — vae.py:232-282."""
         ws, W, hw = self.ws, self.w, h * w
@@ -113,7 +124,7 @@ class VaeEngine:
         qk = ws.get("qk16", (M, 2 * c), self.op_dtype)
         lib.gemm(a16, W[p + "qk.w"], qk, M=M, N=2 * c, K=c, bias=W[p + "qk.b"])
         o16 = ws.get("o16", (M, c), self.op_dtype)
-        rows = min(hw, 8192)
+        rows = min(hw, self.attn_rows(hw))
         for b in range(nb):
             a_b = a16[b * hw:(b + 1) * hw]
             vt = ws.get("vt16", (c, hw), self.op_dtype)               # V^T [C, hw]

@@ -93,6 +93,17 @@ class ControlLDM:
         self._txt_cache = {}
         self._svae = None
 
+    def release_engine_buffers(self) -> None:
+        """Frees the UNet / ControlNet engine's batch-sized buffers and graphs (see CldmEngine.release_buffers)."""
+        if self.engine is not None:
+            self.engine.release_buffers()
+        self._ctx_ref = self._t_key = None
+
+    def release_vae_buffers(self) -> None:
+        """Frees the VAE engine's workspace and graphs (see VaeEngine.release_buffers)."""
+        if self.vae is not None:
+            self.vae.release_buffers()
+
     def _build(self):
         if self.engine is None:
             if self._unet_sd is None or self._cn_sd is None:

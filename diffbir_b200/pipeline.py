@@ -14,7 +14,8 @@ import torch.nn.functional as F
 from . import lib
 from .model import ControlLDM, Diffusion
 from .sampler import DDIMSampler, DPMSolverSampler, EDMSampler, SpacedSampler
-from .utils.common import make_tiled_fn, wavelet_reconstruction
+from .sampler.sampler import tiled_run_chunked
+from .utils.common import make_tiled_fn, sliding_windows, wavelet_reconstruction
 
 
 def resize_short_edge_to(imgs: torch.Tensor, size: int) -> torch.Tensor:
@@ -48,6 +49,7 @@ class Pipeline:
         self.fused_post = True             # colour fix + quantisation as one kernel (False: the torch op sequence)
         self.shard_vae = True              # cooperating ranks (tiled / batch-sharded sampling) shard the VAE by image rows
         self.shard_batch = False           # un-tiled batches: shard (image, CFG branch) forwards over torch.distributed ranks
+        self.max_tile_forwards = 128       # tiled sampling: most tile-forwards x images per graph replay (Sampler.max_tile_forwards)
         self.marks: Optional[list] = None  # set to [] to record (phase, CUDA event) boundaries (bench.py phases_ms)
 
     def _mark(self, name: str) -> None:
@@ -136,12 +138,23 @@ class Pipeline:
         else:
             raise NotImplementedError(sampler_type)
         sampler.shard_batch = self.shard_batch
+        sampler.max_tile_forwards = self.max_tile_forwards
+        if cldm_tiled and tiled_run_chunked(len(sliding_windows(h2, w2, cldm_tile_size // 8, cldm_tile_stride // 8)),
+                                            1 if cfg_scale == 1.0 else 2, bs, self.max_tile_forwards,
+                                            sampler.shard_tiles):
+            # an image too large for one replay: the encoder's full-resolution buffers are not needed again
+            # before the decode, so the sampler's activations get their memory
+            self.cldm.release_vae_buffers()
         z = sampler.sample(model=self.cldm, device=self.device, steps=steps, x_size=(bs, 4, h2, w2),
                            cond=cond, uncond=uncond, cfg_scale=cfg_scale, tiled=cldm_tiled,
                            tile_size=cldm_tile_size // 8, tile_stride=cldm_tile_stride // 8, x_T=x_T,
                            progress=True)
         self.last_sampler = sampler
         self._mark("sampler_loop")
+        if sampler.last_stats.get("chunks", 1) > 1:
+            # only images too large for one replay get here: hand the sampler's activations back so that the
+            # full-resolution decode fits beside them; smaller runs keep their buffers and graphs across calls
+            self.cldm.release_engine_buffers()
         z = z[..., :h1, :w1].contiguous()
         x = self.cldm.vae_decode(z)
         self.cldm.shard_vae = False

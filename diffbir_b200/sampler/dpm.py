@@ -206,7 +206,8 @@ class DPMSolverSampler(Sampler):
         if isinstance(model, ControlLDM):
             ev = EngineEval(model, x_T, cond, uncond if use_cfg else None, tiled, tile_size, tile_stride,
                             shard_tiles=self.shard_tiles, shard_batch=self.shard_batch,
-                            time_collective=self.time_collective)
+                            time_collective=self.time_collective,
+                            max_tile_forwards=self.max_tile_forwards)
             grid = _Multistep.time_grid(ns, steps, "cpu")
             ev.set_timesteps([float(v) for v in ns.model_time(grid[:-1]).tolist()])
             self.last_stats = ev.stats

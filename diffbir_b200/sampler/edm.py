@@ -400,7 +400,8 @@ class EDMSampler(Sampler):
             use_cfg = not (uncond is None or cfg_scale == 1.0)
             ev = EngineEval(model, x_T, cond, uncond if use_cfg else None, tiled, tile_size, tile_stride,
                             shard_tiles=self.shard_tiles, shard_batch=self.shard_batch,
-                            time_collective=self.time_collective)
+                            time_collective=self.time_collective,
+                            max_tile_forwards=self.max_tile_forwards)
             dev = ev.dev
             ev.set_timesteps([int(t) for t in self.timesteps.tolist()])
             self.last_stats = ev.stats

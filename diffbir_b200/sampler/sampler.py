@@ -4,7 +4,8 @@ ddim_sampler.py) with the same constructors and `sample(...)` signature.
 
 When `model` is a diffbir_b200 ControlLDM the loop runs on the kernel engine:
   * cond and uncond branches (and, when tiled, all latent tiles) are ONE batched forward,
-    captured once in a CUDA graph and replayed every step;
+    captured once in a CUDA graph and replayed every step; tiled runs with more tile-forwards than
+    `max_tile_forwards` replay that graph once per chunk of tiles of one branch (bounded memory);
   * text K/V and every time embedding are computed before the loop;
   * CFG mix + x0 + posterior/DDIM update is one fused kernel per step (dbir_sampler_step);
   * tiles are gathered / Gaussian-blended on the device in the reference's accumulation order;
@@ -57,6 +58,44 @@ def assemble_units(recv: torch.Tensor, num_units: int) -> torch.Tensor:
     return recv.transpose(0, 1).reshape(slots * world, *recv.shape[2:])[:num_units].contiguous()
 
 
+def plan_tile_chunks(mine: List[int], num_tiles: int, batch: int,
+                     max_tile_forwards: int) -> Tuple[int, List[Tuple[int, int, int]]]:
+    """Graph replays of one rank's tile-forward units (`mine`: ascending unit ids, unit u = branch * num_tiles
+    + tile, each unit is `batch` batch entries). Returns (units per replay, [(first local slot, units, branch)])
+    with the chunks in local slot order, so writing each chunk's eps at its slots keeps the blend in unit order.
+
+    When every unit fits under `max_tile_forwards` batch entries there is ONE chunk holding all of them
+    (branch -1: it may mix the CFG branches). Otherwise every chunk holds units of one CFG branch, so a replay
+    reads one text context, and each branch's units are spread evenly over the fewest chunks that respect the
+    cap. All chunks replay one graph of the largest chunk's size; a shorter chunk's spare entries keep earlier
+    tiles and their outputs are ignored (batch-invariant plans: they do not touch the other entries' bits)."""
+    if max_tile_forwards < batch:
+        raise ValueError(f"max_tile_forwards ({max_tile_forwards}) is below the batch size ({batch}): "
+                         "one tile-forward of every image must fit into a replay")
+    n = len(mine)
+    if n * batch <= max_tile_forwards:
+        return n, ([(0, n, -1)] if n else [])
+    per = max_tile_forwards // batch
+    chunks, o = [], 0
+    while o < n:
+        br = mine[o] // num_tiles
+        nb_ = sum(1 for u in mine[o:] if u // num_tiles == br)     # this branch's units (contiguous: mine ascends)
+        size = -(-nb_ // -(-nb_ // per))                            # ceil(n / ceil(n / per)) <= per
+        for s in range(o, o + nb_, size):
+            chunks.append((s, min(size, o + nb_ - s), br))
+        o += nb_
+    return max(c for _, c, _ in chunks), chunks
+
+
+def tiled_run_chunked(num_tiles: int, nbr: int, batch: int, max_tile_forwards: int, shard_tiles: bool = True) -> bool:
+    """Whether EngineEval replays this rank's tile-forwards in more than one chunk (same ownership and plan)."""
+    import torch.distributed as dist
+    sharded = shard_tiles and dist.is_available() and dist.is_initialized()
+    world, rank = (dist.get_world_size(), dist.get_rank()) if sharded else (1, 0)
+    mine = tiles_of_rank(nbr * num_tiles, rank, world)
+    return len(plan_tile_chunks(mine, num_tiles, batch, max_tile_forwards)[1]) > 1
+
+
 def _sync_from_rank0(t: torch.Tensor, dev) -> torch.Tensor:
     import torch.distributed as dist
     t = t.to(dev).contiguous()
@@ -99,6 +138,8 @@ class EngineEval:
     captured in a CUDA graph and replayed per evaluation, tile gather / Gaussian blend in the reference's
     accumulation order, and - with torch.distributed initialised - tiles (tiled sampling) or (branch, image)
     units (shard_batch) sharded round-robin over the ranks and re-assembled by one all-gather per evaluation.
+    Tiled sampling with more than `max_tile_forwards` batch entries on a rank replays the graph once per chunk
+    (plan_tile_chunks); the result has the same bits as one replay of all of them.
 
         ev = EngineEval(model, x_T, cond, uncond, tiled, tile_size, tile_stride)
         ev.set_timesteps([999, 979, ...])      # every model timestep the loop will ask for (floats allowed)
@@ -108,7 +149,7 @@ class EngineEval:
     condition and noise stream, otherwise tiles of diverging latents would be blended silently)."""
 
     def __init__(self, model, x_T, cond, uncond, tiled=False, tile_size=-1, tile_stride=-1, *, shard_tiles=True,
-                 shard_batch=False, time_collective=False):
+                 shard_batch=False, time_collective=False, max_tile_forwards=128):
         import torch.distributed as dist
         model._build()
         self.model, self.eng = model, model.engine
@@ -131,6 +172,7 @@ class EngineEval:
             _sync_rng_from_rank0(dev)
         self.x0 = x
         T = Tl = 0
+        self.chunked = False
         if tiled:
             # unit u = branch * T + tile: the nbr * T tile-forwards of one evaluation are owned round-robin
             # (u % world). Sharding (tile, CFG branch) units instead of whole tiles keeps the ranks within one
@@ -151,20 +193,39 @@ class EngineEval:
                 self.branch_tiles.append((o, len(tj), self.all_coords[tj].contiguous() if tj else self.all_coords[:0]))
                 o += len(tj)
             self.wts = torch.tensor(gaussian_weights(ts_, ts_), dtype=torch.float32, device=dev)
-            nb = Ul * B
-            c_img = torch.empty(max(Ul, 1) * B, C, ts_, ts_, device=dev)[:nb]
+            # The tile-forwards of one evaluation are replayed in chunks of at most max_tile_forwards batch
+            # entries, so the engine's activations stay bounded whatever the image size (one chunk up to the cap).
+            per_chunk, self.chunks = plan_tile_chunks(mine, T, B, max_tile_forwards)
+            self.chunked = len(self.chunks) > 1
+            c_img = torch.empty(max(Ul, 1) * B, C, ts_, ts_, device=dev)[:Ul * B]
             ctx_parts = []
             for (o, nj, coords), cd in zip(self.branch_tiles, conds):
                 if nj:
                     lib.tile_gather(cd["c_img"].to(dev, torch.float32).contiguous(), B, C, H, W, coords, nj, ts_,
                                     c_img[o * B:(o + nj) * B])
-                    ctx_parts.append(cd["c_txt"].to(dev, torch.float32).expand(B, -1, -1).repeat(nj, 1, 1))
-            ctx = torch.cat(ctx_parts, 0) if ctx_parts else None
+                    if not self.chunked:
+                        ctx_parts.append(cd["c_txt"].to(dev, torch.float32).expand(B, -1, -1).repeat(nj, 1, 1))
+            if self.chunked:
+                # pad the replay to a size the engine runs as grouped twin launches where the cap allows it,
+                # so chunked runs take the same forward path as the single replay of a smaller image
+                per_chunk = next((n for n in range(per_chunk, max_tile_forwards // B + 1)
+                                  if eng.twins_feasible(n * B, ts_, ts_)), per_chunk)
+                # branch-pure chunks: one text context per branch, its cross-attention K/V built once per run
+                self.unit_coords = self.all_coords[[u % T for u in mine]].contiguous()
+                self.ctx_layouts = {jb: conds[jb]["c_txt"].to(dev, torch.float32).expand(B, -1, -1)
+                                    .repeat(per_chunk, 1, 1) for jb in sorted({c[2] for c in self.chunks})}
+                self.c_img_units = c_img
+                nb, ctx = per_chunk * B, None
+            else:
+                nb = Ul * B
+                ctx = torch.cat(ctx_parts, 0) if ctx_parts else None
             gh = gw = ts_
             Tl = Ul                                            # (stats) tile-forwards of this rank
             if world > 1:
                 self.send = torch.zeros(slots, B, C, ts_, ts_, device=dev)
                 self.recv = torch.empty(world, slots, B, C, ts_, ts_, device=dev)
+            if self.chunked:                                   # eps of every local unit, in local slot order
+                self.eps_units = self.send[:Ul] if world > 1 else torch.empty(Ul, B, C, ts_, ts_, device=dev)
             self.eps_full = torch.empty(nbr, B, C, H, W, device=dev)
         elif world > 1:
             # batch sharding: unit u = branch * B + image, owned round-robin like tiles (u % world)
@@ -194,7 +255,8 @@ class EngineEval:
         eng.batch_invariant = bool(tiled) or world > 1 or eng.deterministic
         self.graph = None
         self.stats = dict(world=world, tiles=T, units_this_rank=Tl, forwards_per_step=nb,
-                          batch_sharded=bool(world > 1 and not tiled))
+                          batch_sharded=bool(world > 1 and not tiled),
+                          chunks=len(self.chunks) if tiled else int(nb > 0))
 
     def set_timesteps(self, model_ts) -> None:
         """Time embeddings of every timestep the loop will evaluate + the CUDA graph of the forward."""
@@ -202,13 +264,23 @@ class EngineEval:
         self.model_ts = list(model_ts)
         if self.nb > 0:
             B, C, H, W = self.shape
-            eng.set_context(self._ctx)
+            if self.chunked:
+                # K/V of each branch's context, kept aside and copied into the engine's static buffers
+                # whenever the next chunk belongs to the other branch
+                self.kv_layouts = {}
+                for jb, ctx in self.ctx_layouts.items():
+                    eng.set_context(ctx)
+                    self.kv_layouts[jb] = {k: v.clone() for k, v in eng.kv.items() if k.startswith("g")}
+                self.kv_cur = jb
+            else:
+                eng.set_context(self._ctx)
             eng.set_timesteps(self.model_ts, self.nb)
             self.model._ctx_ref = self.model._t_key = None      # generic-path caches are now stale
             eng.load_step(0)
-            self.graph, self.x_in, c_img_buf, self.out, self.graph_launches = eng.graphed_forward(
+            self.graph, self.x_in, self.c_img_in, self.out, self.graph_launches = eng.graphed_forward(
                 self.nb, C, self.gh, self.gw, self.scales)
-            c_img_buf.copy_(self._c_img)
+            if not self.chunked:
+                self.c_img_in.copy_(self._c_img)
 
     def _fill_inputs(self, x: torch.Tensor) -> None:
         B, C, H, W = self.shape
@@ -224,6 +296,23 @@ class EngineEval:
             for j in range(nbr):
                 v[j].copy_(x)
 
+    def _replay_chunks(self, x: torch.Tensor, step_idx: int) -> None:
+        """One evaluation as several replays of the chunk graph; each writes its units' eps to their local slots."""
+        B, C, H, W = self.shape
+        ts = self.ts
+        self.eng.load_step(step_idx)
+        # chunks of the branch whose K/V is loaded go first: one K/V switch per evaluation
+        for s, n, jb in sorted(self.chunks, key=lambda c: c[2] != self.kv_cur):
+            if jb != self.kv_cur:
+                for k, v in self.kv_layouts[jb].items():
+                    self.eng.kv[k].copy_(v)
+                self.kv_cur = jb
+            lib.tile_gather(x, B, C, H, W, self.unit_coords[s:s + n], n, ts, self.x_in[:n * B])
+            self.c_img_in[:n * B].copy_(self.c_img_units[s * B:(s + n) * B])
+            self.graph.replay()
+            lib.count_launch(self.graph_launches)
+            self.eps_units[s:s + n].copy_(self.out[:n * B].view(n, B, C, ts, ts))
+
     def _all_gather(self) -> None:
         if self.time_collective:
             ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -237,19 +326,21 @@ class EngineEval:
         """(cond, uncond | None) model outputs for the full latent x at model_ts[step_idx], fp32 [B,C,H,W]."""
         B, C, H, W = self.shape
         nbr, world = self.nbr, self.world
-        if self.nb > 0:
+        if self.chunked:
+            self._replay_chunks(x, step_idx)
+        elif self.nb > 0:
             self.eng.load_step(step_idx)
             self._fill_inputs(x)
             self.graph.replay()
             lib.count_launch(self.graph_launches)
         if self.tiled:
             if world > 1:
-                if self.Ul:
+                if self.Ul and not self.chunked:
                     self.send[:self.Ul].copy_(self.out.view(self.Ul, B, C, self.ts, self.ts))
                 self._all_gather()
                 tiles = assemble_units(self.recv, nbr * self.T).view(nbr, self.T, B, C, self.ts, self.ts)
             else:
-                tiles = self.out.view(nbr, self.T, B, C, self.ts, self.ts)
+                tiles = (self.eps_units if self.chunked else self.out).view(nbr, self.T, B, C, self.ts, self.ts)
             for j in range(nbr):
                 lib.tile_blend(tiles[j], B, C, H, W, self.all_coords, self.T, self.ts, self.wts, self.eps_full[j])
             ev = self.eps_full
@@ -277,6 +368,10 @@ class Sampler:
         # all-gather of eps per step (BASELINE configs[4]: 4 images x 2 branches -> one forward per GPU of
         # an 8-GPU box). Opt-in: ranks that restore DIFFERENT images (independent replicas) must not shard.
         self.shard_batch = False
+        # tiled sampling: the most batch entries (tile-forwards x images) one graph replay may hold. More units
+        # than that run as several replays per evaluation, so memory stops growing with the image size; the
+        # 49-tile (98-forward) 2048^2 restoration still takes one replay.
+        self.max_tile_forwards = 128
         self.last_stats: dict = {}
 
     def get_cfg_scale(self, default_cfg_scale: float, model_t: int) -> float:
@@ -315,7 +410,8 @@ class Sampler:
                        tile_stride):
         use_cfg = not (uncond is None or cfg_scale == 1.0)
         ev = EngineEval(model, x_T, cond, uncond if use_cfg else None, tiled, tile_size, tile_stride,
-                        shard_tiles=self.shard_tiles, shard_batch=self.shard_batch, time_collective=self.time_collective)
+                        shard_tiles=self.shard_tiles, shard_batch=self.shard_batch, time_collective=self.time_collective,
+                        max_tile_forwards=self.max_tile_forwards)
         x = ev.x0
         coefs = coefs.to(ev.dev)
         order = list(range(len(ts)))[::-1]                     # table index of each loop iteration

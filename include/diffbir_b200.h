@@ -97,7 +97,8 @@ int64_t dbir_attention_ws_bytes(int32_t batch, int32_t heads, int32_t sq, int32_
 /* ---- GroupNorm (32 groups) / LayerNorm ------------------------------------------------
  * dbir_gn_stats: per-(image, group) mean and rstd of the virtual concat [src1 | src2] (fp32
  * NHWC, c2 may be 0) -> stats[n][32][2]. workspace: dbir_gn_workspace_floats() floats,
- * zero-initialised once by the caller. Replaces the statistics half of GroupNorm32
+ * zero-initialised once by the caller; its layout is per image, so one workspace sized for the
+ * largest batch serves calls of any smaller batch. Replaces the statistics half of GroupNorm32
  * (util.py:191-193, eps 1e-5) / Normalize (attention.py:48-51, vae.py:18-21, eps 1e-6) and
  * the torch.cat before output-block ResBlocks (controlnet.py:39-44).
  * dbir_gn_apply: out = silu?(gn(x)) as op16 NHWC, optionally 2x nearest-upsampled
