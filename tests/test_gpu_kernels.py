@@ -248,6 +248,18 @@ def test_sampler_step_and_tiles_bit_exact(L, golden_dir):
     x0 = (x - coef[1] * e2) / coef[0]
     ref = coef[2] * x0 + coef[3] * e2 + coef[4] * nz
     assert torch.equal(out, ref)
+    # modes 1 (spaced, v: same update as mode 0) and 2 (DDIM, eps), each also without CFG (eps_uncond NULL)
+    # and without noise (NULL: the last step)
+    for ecu in (eu, None):
+        for noise in (nz, None):
+            e = ec if ecu is None else ecu + 4.0 * (ec - ecu)
+            n_ = torch.zeros_like(x) if noise is None else noise
+            L.sampler_step(ec, ecu, 4.0, x, noise, coef, 1, x.numel(), out)
+            x0 = coef[0] * x - coef[1] * e
+            assert torch.equal(out, (coef[2] * x0 + coef[3] * x) + coef[4] * n_)
+            L.sampler_step(ec, ecu, 4.0, x, noise, coef, 2, x.numel(), out)
+            x0 = (x - coef[1] * e) / coef[0]
+            assert torch.equal(out, coef[2] * x0 + coef[3] * e + coef[4] * n_)
     # tile gather / blend against the reference-order accumulation of the oracle
     H, W, ts, stride = 24, 40, 16, 8
     wins = osm.sliding_windows(H, W, ts, stride)

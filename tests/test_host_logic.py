@@ -279,3 +279,79 @@ def test_diffbir_alias_exposes_the_reference_names():
     from diffbir.model.gaussian_diffusion import Diffusion
     from diffbir.model.swinir import SwinIR
     assert ControlLDM is dm.ControlLDM and Diffusion is dm.Diffusion and SwinIR is dm.SwinIR
+
+
+# ---- coverage guard: every compute entry point and every GEMM option is exercised by a GPU test ----------------
+_NOT_COMPUTE = {"dbir_version", "dbir_last_error", "dbir_operand_kind", "dbir_sm_count", "dbir_gemm_gn_slots",
+                "dbir_gemm_model_plan"}
+# dbir_gemm_args options and the lib.gemm default that leaves each one off
+_GEMM_OPTION_DEFAULTS = {"lda": 0, "ldb": 0, "ldr": None, "ldo": None, "rows_per_vec": 0, "rowvec": None,
+                         "bias_per_row": False, "alpha": 1.0, "geglu": False, "groups": 1, "split_k": 0,
+                         "cta_pair": 0, "force_bn": 0, "gn_partials": None, "gn_rows_per_img": 0}
+
+
+def _compute_entry_points():
+    import re
+    src = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / "diffbir_b200.h").read_text(), flags=re.S)
+    names = sorted(set(re.findall(r"\b(dbir_\w+)\s*\(", src)))
+    return [n for n in names if n not in _NOT_COMPUTE and not n.endswith(("_ws_bytes", "_workspace_floats"))]
+
+
+def _lib_calls(paths):
+    """(module path, ast.Call) of every `L.<fn>(...)` / `lib.<fn>(...)` call in the given test modules."""
+    import ast
+    for path in paths:
+        tree = ast.parse(path.read_text())
+        for node in ast.walk(tree):
+            if (isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute)
+                    and isinstance(node.func.value, ast.Name) and node.func.value.id in ("L", "lib")):
+                yield path, tree, node
+
+
+def test_every_compute_entry_point_has_a_gpu_test():
+    """Each compute function of include/diffbir_b200.h is called through its lib wrapper by a tests/test_gpu_*.py
+    module, so a new entry point cannot land without a kernel-level test."""
+    import inspect
+    from diffbir_b200 import lib
+    entry = _compute_entry_points()
+    assert "dbir_gemm" in entry and "dbir_window_attention" in entry and len(entry) >= 20
+    called = {node.func.attr for _, _, node in _lib_calls(sorted((ROOT / "tests").glob("test_gpu_*.py")))}
+    missing = []
+    for name in entry:
+        fn = name[len("dbir_"):]
+        wrapper = getattr(lib, fn, None)
+        assert wrapper is not None and name in inspect.getsource(wrapper), f"lib.{fn} does not wrap {name}"
+        if fn not in called:
+            missing.append(name)
+    assert not missing, f"entry points no GPU test calls: {missing}"
+
+
+def test_every_gemm_option_is_exercised():
+    """Each dbir_gemm option is passed with a non-default value by some test under tests/, and every lib.ACT
+    activation is requested: literally (act="silu") or, where a test loops over activations, as a string in a
+    tuple / list of that module."""
+    import ast
+    from diffbir_b200 import lib
+    seen, acts = set(), set()
+    for _, tree, node in _lib_calls(sorted((ROOT / "tests").glob("*.py"))):
+        if node.func.attr != "gemm":
+            continue
+        for kw in node.keywords:
+            if kw.arg is None:
+                continue
+            literal = isinstance(kw.value, ast.Constant)
+            if kw.arg == "act":
+                if literal:
+                    acts.add(lib.ACT[kw.value.value])
+                else:                                   # looped: the ACT names listed in this module's tuples
+                    for seq in ast.walk(tree):
+                        if isinstance(seq, (ast.Tuple, ast.List)):
+                            for leaf in ast.walk(seq):
+                                if isinstance(leaf, ast.Constant) and isinstance(leaf.value, str) and leaf.value in lib.ACT:
+                                    acts.add(lib.ACT[leaf.value])
+            elif kw.arg in _GEMM_OPTION_DEFAULTS:
+                if not literal or kw.value.value != _GEMM_OPTION_DEFAULTS[kw.arg]:
+                    seen.add(kw.arg)
+    assert set(lib.ACT.values()) <= acts, f"activations no test requests: {set(lib.ACT.values()) - acts}"
+    missing = set(_GEMM_OPTION_DEFAULTS) - seen
+    assert not missing, f"dbir_gemm options no test sets: {sorted(missing)}"
