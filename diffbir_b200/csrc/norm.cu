@@ -232,6 +232,94 @@ gn_finalize_kernel(const float* __restrict__ p1, int slots1, int c1, const float
   }
 }
 
+// ---- Tiled-VAE GroupNorm (reference utils/tilevae/tilevae.py, non-fast mode) ----
+// Every tile of an image is normalised with one shared (mean, var) per group: the pixel-weighted average of
+// the tiles' own means and biased variances (no between-tile variance term). dbir_gn_moments takes each tile's
+// (mean, var) per (batch entry, group); dbir_gn_merge combines them.
+
+// Per-slot column sums of a fp32 NHWC tensor in the dbir_gemm gn_partials layout [n][slots][c][2], 32 pixels a
+// slot, for tensors written by kernels without the fused epilogue. grid = (slots, n).
+__global__ void __launch_bounds__(128)
+gn_col_partials_kernel(const float* __restrict__ x, int hw, int c, int slots, float* __restrict__ part) {
+  pdl_trigger();
+  pdl_wait();
+  const int slot = blockIdx.x, n = blockIdx.y;
+  const int p0 = slot * 32, p1 = min(hw, p0 + 32);
+  for (int ch = threadIdx.x; ch < c; ch += blockDim.x) {
+    float s = 0.f, q = 0.f;
+    for (int p = p0; p < p1; ++p) {
+      const float v = x[(static_cast<long long>(n) * hw + p) * c + ch];
+      s += v;
+      q += v * v;
+    }
+    *reinterpret_cast<float2*>(part + ((static_cast<long long>(n) * slots + slot) * c + ch) * 2) = make_float2(s, q);
+  }
+}
+
+// (mean, biased var) per (batch entry, group) from slot partials, fp64, fixed order. grid = (32, n).
+// Entry j of the batch is written at moments[entry ? entry[j] : entry0 + j].
+__global__ void __launch_bounds__(FIN_THREADS)
+gn_moments_kernel(const float* __restrict__ part, int slots, int c, int hw, const int* __restrict__ entry, int entry0,
+                  double* __restrict__ moments) {
+  pdl_trigger();
+  pdl_wait();
+  const int g = blockIdx.x, n = blockIdx.y, cpg = c / 32;
+  double a = 0.0, b = 0.0;
+  fin_accumulate<1>(part + static_cast<long long>(n) * slots * c * 2, c, g * cpg, cpg, cpg * slots, 0, a, b);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    b += __shfl_xor_sync(0xffffffffu, b, o);
+  }
+  __shared__ double sa[FIN_THREADS / 32], sb[FIN_THREADS / 32];
+  if ((threadIdx.x & 31) == 0) { sa[threadIdx.x >> 5] = a; sb[threadIdx.x >> 5] = b; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double ta = 0.0, tb = 0.0;
+#pragma unroll
+    for (int i = 0; i < FIN_THREADS / 32; ++i) { ta += sa[i]; tb += sb[i]; }
+    const double cnt = static_cast<double>(hw) * cpg;
+    const double mean = ta / cnt;
+    double var = tb / cnt - mean * mean;
+    if (var < 0.0) var = 0.0;
+    const long long e = entry ? entry[n] : entry0 + n;
+    moments[(e * 32 + g) * 2 + 0] = mean;
+    moments[(e * 32 + g) * 2 + 1] = var;
+  }
+}
+
+// One thread per (image, group): the pixel-weighted mean of the moments of that image's entries, visited in
+// entry order (reverse = 1: backwards), then (mean, rstd) written for each of those entries.
+__global__ void __launch_bounds__(128)
+gn_merge_kernel(const double* __restrict__ moments, const long long* __restrict__ pixels, const int* __restrict__ image,
+                int entries, int images, int reverse, float eps, float* __restrict__ stats) {
+  pdl_trigger();
+  pdl_wait();
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= images * 32) return;
+  const int img = idx / 32, g = idx % 32;
+  double total = 0.0;
+  for (int i = 0; i < entries; ++i) {
+    const int e = reverse ? entries - 1 - i : i;
+    if (image[e] == img) total += static_cast<double>(pixels[e]);
+  }
+  double mean = 0.0, var = 0.0;
+  for (int i = 0; i < entries; ++i) {
+    const int e = reverse ? entries - 1 - i : i;
+    if (image[e] != img) continue;
+    const double wt = static_cast<double>(pixels[e]) / total;
+    mean += wt * moments[(static_cast<long long>(e) * 32 + g) * 2 + 0];
+    var += wt * moments[(static_cast<long long>(e) * 32 + g) * 2 + 1];
+  }
+  const float m = static_cast<float>(mean);
+  const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+  for (int e = 0; e < entries; ++e) {
+    if (image[e] != img) continue;
+    stats[(static_cast<long long>(e) * 32 + g) * 2 + 0] = m;
+    stats[(static_cast<long long>(e) * 32 + g) * 2 + 1] = rstd;
+  }
+}
+
 // Stage 2: y = silu?(x * a[c] + b[c]) -> op16, optional 2x nearest upsample, optional raw copy.
 // grid = (pixel chunks, N)
 __global__ void __launch_bounds__(256)
@@ -430,6 +518,36 @@ extern "C" int dbir_gn_finalize(const float* partials1, int32_t slots1, int32_t 
     default: DBIR_FIN(8); break;
   }
 #undef DBIR_FIN
+  return 0;
+}
+
+extern "C" int64_t dbir_gn_moments_workspace_floats(int32_t n, int32_t hw, int32_t c) {
+  return static_cast<int64_t>(n) * ((hw + 31) / 32) * c * 2;
+}
+
+extern "C" int dbir_gn_moments(const float* partials, int32_t slots, const float* x, int32_t c, int32_t n, int32_t hw,
+                               float* workspace, const int32_t* entry, int32_t entry0, double* moments, void* stream) {
+  DBIR_REQUIRE(moments && n > 0 && hw > 0 && c % 32 == 0, "dbir_gn_moments: bad args");
+  DBIR_REQUIRE((partials && slots > 0) != (x != nullptr), "dbir_gn_moments: exactly one of partials / x");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (x) {
+    DBIR_REQUIRE(workspace, "dbir_gn_moments: x needs a workspace");
+    slots = (hw + 31) / 32;
+    DBIR_CHECK_CUDA(dbir_launch(gn_col_partials_kernel, dim3(slots, n), dim3(128), 0, st, x, hw, c, slots, workspace));
+    partials = workspace;
+  }
+  DBIR_CHECK_CUDA(dbir_launch(gn_moments_kernel, dim3(32, n), dim3(FIN_THREADS), 0, st, partials, slots, c, hw,
+                              entry, entry0, moments));
+  return 0;
+}
+
+extern "C" int dbir_gn_merge(const double* moments, const int64_t* pixels, const int32_t* image, int32_t entries,
+                             int32_t images, int32_t reverse, float eps, float* stats, void* stream) {
+  DBIR_REQUIRE(moments && pixels && image && stats && entries > 0 && images > 0, "dbir_gn_merge: bad args");
+  const int threads = images * 32;
+  DBIR_CHECK_CUDA(dbir_launch(gn_merge_kernel, dim3((threads + 127) / 128), dim3(128), 0,
+                              reinterpret_cast<cudaStream_t>(stream), moments,
+                              reinterpret_cast<const long long*>(pixels), image, entries, images, reverse, eps, stats));
   return 0;
 }
 

@@ -203,6 +203,26 @@ def gn_stats(src1, src2, c1, c2, n, hw, eps, stats, workspace):
     count_launch()
 
 
+def gn_moments_workspace_floats(n, hw, c) -> int:
+    lib = load()
+    lib.dbir_gn_moments_workspace_floats.restype = C.c_int64
+    return int(lib.dbir_gn_moments_workspace_floats(n, hw, c))
+
+
+def gn_moments(c, n, hw, moments, *, partials=None, slots=0, x=None, workspace=None, entry=None, entry0=0):
+    """fp64 (mean, biased var) per (batch entry, group) of GEMM partial sums or a fp32 NHWC tensor x."""
+    check(load().dbir_gn_moments(_fp(partials), slots, _fp(x), c, n, hw, _fp(workspace), _fp(entry), entry0,
+                                 _fp(moments), _sp()), "dbir_gn_moments")
+    count_launch(1 if x is None else 2)
+
+
+def gn_merge(moments, pixels, image, entries, images, stats, *, reverse=False, eps=1e-6):
+    """Tiled-VAE GroupNorm statistics: pixel-weighted mean of the entries' moments per (image, group)."""
+    check(load().dbir_gn_merge(_fp(moments), _fp(pixels), _fp(image), entries, images, 1 if reverse else 0,
+                               C.c_float(eps), _fp(stats), _sp()), "dbir_gn_merge")
+    count_launch()
+
+
 def gn_apply(src1, src2, c1, c2, n, h, w, stats, gamma, beta, out, *, norm=True, silu=True,
              upsample=1, out_raw=None, imgs_per_group=0):
     check(load().dbir_gn_apply(_fp(src1), _fp(src2), c1, c2, n, h, w, _fp(stats), _fp(gamma),

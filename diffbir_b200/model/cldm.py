@@ -49,6 +49,7 @@ class ControlLDM:
         # the same tensors; set by the pipeline while ranks cooperate on one job: tiled / batch-sharded sampling)
         self.shard_vae = False
         self._svae = None
+        self._tvae = None
 
     # --------------------------------------------------------------- checkpoint loaders
     @torch.no_grad()
@@ -91,7 +92,7 @@ class ControlLDM:
         self.engine = self.vae = self.clip = None
         self._ctx_ref = self._t_key = None
         self._txt_cache = {}
-        self._svae = None
+        self._svae = self._tvae = None
 
     def release_engine_buffers(self) -> None:
         """Frees the UNet / ControlNet engine's batch-sized buffers and graphs (see CldmEngine.release_buffers)."""
@@ -100,9 +101,11 @@ class ControlLDM:
         self._ctx_ref = self._t_key = None
 
     def release_vae_buffers(self) -> None:
-        """Frees the VAE engine's workspace and graphs (see VaeEngine.release_buffers)."""
+        """Frees the VAE engine's workspace and graphs (see VaeEngine.release_buffers), tiled VAE included."""
         if self.vae is not None:
             self.vae.release_buffers()
+        if self._tvae is not None:
+            self._tvae.release_buffers()
 
     def _build(self):
         if self.engine is None:
@@ -166,12 +169,14 @@ class ControlLDM:
     @torch.no_grad()
     def vae_encode(self, image: torch.Tensor, sample: bool = True, tiled: bool = False,
                    tile_size: int = -1) -> torch.Tensor:
+        """tiled: the reference's Tiled-VAE semantics (engine.vae_tiled), tile_size in image pixels."""
         self._build()
-        if tiled:
-            raise NotImplementedError("tiled VAE (utils/tilevae) is outside the hot path: the VAE engines run un-tiled")
         image = image.to(self.device, torch.float32).contiguous()
-        sv = self._sharded_vae(image.shape[2], image.shape[3])
-        m = sv.encode_moments(image) if sv is not None else self.vae.encode_moments(image)
+        if tiled:
+            m = self.tiled_vae().encode_moments(image, tile_size)
+        else:
+            sv = self._sharded_vae(image.shape[2], image.shape[3])
+            m = sv.encode_moments(image) if sv is not None else self.vae.encode_moments(image)
         mean, logvar = m.chunk(2, dim=1)
         if sample:   # DiagonalGaussianDistribution.sample, model/distributions.py:25-37
             std = torch.exp(0.5 * torch.clamp(logvar, -30.0, 20.0))
@@ -180,12 +185,22 @@ class ControlLDM:
 
     @torch.no_grad()
     def vae_decode(self, z: torch.Tensor, tiled: bool = False, tile_size: int = -1) -> torch.Tensor:
+        """tiled: the reference's Tiled-VAE semantics (engine.vae_tiled), tile_size in latent pixels."""
         self._build()
-        if tiled:
-            raise NotImplementedError("tiled VAE (utils/tilevae) is outside the hot path: the VAE engines run un-tiled")
         z = (z / self.scale_factor).to(self.device, torch.float32).contiguous()
+        if tiled:
+            return self.tiled_vae().decode(z, tile_size)
         sv = self._sharded_vae(8 * z.shape[2], 8 * z.shape[3])
         return sv.decode(z) if sv is not None else self.vae.decode(z)
+
+    def tiled_vae(self):
+        """The tiled VAE (engine.vae_tiled) on this model's VAE weights. It runs on each rank by itself: the
+        row-sharded VAE computes the un-tiled semantics."""
+        self._build()
+        if self._tvae is None:
+            from ..engine.vae_tiled import TiledVae
+            self._tvae = TiledVae(self.vae)
+        return self._tvae
 
     def _sharded_vae(self, h_img: int, w_img: int):
         """The row-sharded VAE (engine.vae_sharded) when ranks cooperate on this job and the size allows it."""
@@ -206,14 +221,15 @@ class ControlLDM:
                     c_img=self.vae_encode(cond_img * 2 - 1, sample=False, tiled=tiled, tile_size=tile_size))
 
     @torch.no_grad()
-    def prepare_condition_pair(self, cond_img: torch.Tensor, pos_txt: List[str], neg_txt: List[str]):
+    def prepare_condition_pair(self, cond_img: torch.Tensor, pos_txt: List[str], neg_txt: List[str],
+                               tiled: bool = False, tile_size: int = -1):
         """(cond, uncond) of Pipeline.apply_cldm (pipeline.py:116-128): the condition image is encoded
         once (the posterior mode is deterministic, the reference encodes the same image twice) and both
         prompt lists share one batched text-tower call."""
         self._build()
         n = len(pos_txt)
         c_txt = self.encode_text(list(pos_txt) + list(neg_txt))
-        c_img = self.vae_encode(cond_img * 2 - 1, sample=False)
+        c_img = self.vae_encode(cond_img * 2 - 1, sample=False, tiled=tiled, tile_size=tile_size)
         return (dict(c_txt=c_txt[:n].contiguous(), c_img=c_img),
                 dict(c_txt=c_txt[n:].contiguous(), c_img=c_img.clone()))
 

@@ -37,6 +37,22 @@ def pad_to_multiples_of(imgs: torch.Tensor, multiple: int) -> torch.Tensor:
     return F.pad(imgs, pad=(0, pw, 0, ph), mode="constant", value=0)
 
 
+def vae_tiling(img_hw, enc_tiled: bool, enc_tile: int, dec_tiled: bool, dec_tile: int) -> Tuple[bool, bool]:
+    """Whether the VAE encode / decode of an (already padded) condition image of size img_hw run tiled
+    (pipeline.py:105-115, 219-224): off for inputs smaller than a tile; an encoder tile size that is not a
+    multiple of 8 is refused."""
+    h, w = img_hw
+    if enc_tiled and (h < enc_tile or w < enc_tile):
+        print("[VAE Encoder]: the input size is tiny and unnecessary to tile.")
+        enc_tiled = False
+    if enc_tiled and enc_tile % 8 != 0:
+        raise ValueError("VAE encoder tile size must be a multiple of 8")
+    if dec_tiled and (h // 8 < dec_tile // 8 or w // 8 < dec_tile // 8):
+        print("[VAE Decoder]: the input size is tiny and unnecessary to tile.")
+        dec_tiled = False
+    return enc_tiled, dec_tiled
+
+
 class Pipeline:
     def __init__(self, cleaner, cldm: ControlLDM, diffusion: Diffusion, cond_fn, device: str) -> None:
         self.cleaner = cleaner
@@ -82,24 +98,18 @@ class Pipeline:
         """pipeline.py:71-233."""
         bs, _, h0, w0 = cond_img.shape
         cond_img = pad_to_multiples_of(cond_img, multiple=64 if not vae_encoder_tiled and not cldm_tiled else 8)
-        # Tiled-VAE itself is outside the path (the VAE engines run un-tiled), but the reference switches it off for inputs smaller than
-        # a tile (pipeline.py:106-110, 219-223) and then only the padding rule above differs: that branch is honoured.
-        if vae_encoder_tiled and (cond_img.size(2) < vae_encoder_tile_size or cond_img.size(3) < vae_encoder_tile_size):
-            print("[VAE Encoder]: the input size is tiny and unnecessary to tile.")
-            vae_encoder_tiled = False
-        if vae_decoder_tiled and (cond_img.size(2) // 8 < vae_decoder_tile_size // 8 or cond_img.size(3) // 8 < vae_decoder_tile_size // 8):
-            print("[VAE Decoder]: the input size is tiny and unnecessary to tile.")
-            vae_decoder_tiled = False
-        if vae_encoder_tiled or vae_decoder_tiled:
-            raise NotImplementedError("tiled VAE is outside the hot path: the VAE engines run un-tiled")
-        # ranks that cooperate on this job (sharded tiles or batch units) also shard the VAE by image rows
+        vae_encoder_tiled, vae_decoder_tiled = vae_tiling(cond_img.shape[2:], vae_encoder_tiled, vae_encoder_tile_size,
+                                                          vae_decoder_tiled, vae_decoder_tile_size)
+        # ranks that cooperate on this job (sharded tiles or batch units) also shard the un-tiled VAE by image rows;
+        # a tiled VAE runs replicated on every rank (ControlLDM)
         import torch.distributed as dist
         coop = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and (cldm_tiled or self.shard_batch)
         self.cldm.shard_vae = bool(coop and self.shard_vae)
         # The reference encodes the (identical) condition image twice (pipeline.py:117-128);
         # the latent is deterministic (posterior mode), so it is encoded once and shared.
         # Both prompts go through the text tower as one batch (pipeline.py:117-128 runs it twice).
-        cond, uncond = self.cldm.prepare_condition_pair(cond_img, [pos_prompt] * bs, [neg_prompt] * bs)
+        enc_tiling = dict(tiled=True, tile_size=vae_encoder_tile_size) if vae_encoder_tiled else {}
+        cond, uncond = self.cldm.prepare_condition_pair(cond_img, [pos_prompt] * bs, [neg_prompt] * bs, **enc_tiling)
         self._mark("encode+clip")
         h1, w1 = cond["c_img"].shape[2:]
         if cldm_tiled and (h1 < cldm_tile_size // 8 or w1 < cldm_tile_size // 8):
@@ -151,12 +161,15 @@ class Pipeline:
                            progress=True)
         self.last_sampler = sampler
         self._mark("sampler_loop")
-        if sampler.last_stats.get("chunks", 1) > 1:
-            # only images too large for one replay get here: hand the sampler's activations back so that the
-            # full-resolution decode fits beside them; smaller runs keep their buffers and graphs across calls
+        if sampler.last_stats.get("chunks", 1) > 1 or vae_decoder_tiled:
+            # only images too large for one replay (or for the un-tiled decode) get here: hand the sampler's
+            # activations back so that the full-resolution decode fits beside them -- a tiled decode keeps as much
+            # of its state on the device as half the free memory allows; smaller runs keep their buffers and
+            # graphs across calls
             self.cldm.release_engine_buffers()
         z = z[..., :h1, :w1].contiguous()
-        x = self.cldm.vae_decode(z)
+        dec_tiling = dict(tiled=True, tile_size=vae_decoder_tile_size // 8) if vae_decoder_tiled else {}
+        x = self.cldm.vae_decode(z, **dec_tiling)
         self.cldm.shard_vae = False
         self._mark("vae_decode")
         x = x[:, :, :h0, :w0]

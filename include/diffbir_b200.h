@@ -123,6 +123,21 @@ int dbir_gn_apply(const float* src1, const float* src2, int32_t c1, int32_t c2, 
 int dbir_layernorm(const float* x, int64_t ldx, int32_t rows, int32_t c, const float* gamma,
                    const float* beta, float eps, void* out, int64_t ldo, int32_t out_kind,
                    int32_t rows_per_group, void* stream);   /* out_kind 0 = fp32, 1 = op16 */
+/* Tiled-VAE GroupNorm (non-fast mode of the reference's utils/tilevae/tilevae.py:177-278): each tile of an
+ * image is normalised with the pixel-weighted average of the tiles' own per-group means and biased variances.
+ * dbir_gn_moments: fp64 (mean, biased var) per (batch entry, group) -> moments[e][32][2] at e = entry[j]
+ *   (device int32 [n]) or entry0 + j when entry is NULL. The source is either the partial sums a conv-mode
+ *   dbir_gemm emitted (partials [n][slots][c][2], x NULL) or a fp32 NHWC tensor x [n][hw][c] (partials NULL;
+ *   workspace: dbir_gn_moments_workspace_floats() floats, no initialisation needed).
+ * dbir_gn_merge: for every image, the weights pixels[e] / sum of its entries' pixels, mean = sum w * mean_e,
+ *   var = sum w * var_e (fp64, entries visited in index order, or backwards when reverse = 1) -> (mean, rstd)
+ *   of every entry of that image in the stats[e][32][2] layout dbir_gn_apply reads. image: device int32
+ *   [entries] in [0, images); pixels: device int64 [entries]. Deterministic. */
+int64_t dbir_gn_moments_workspace_floats(int32_t n, int32_t hw, int32_t c);
+int dbir_gn_moments(const float* partials, int32_t slots, const float* x, int32_t c, int32_t n, int32_t hw,
+                    float* workspace, const int32_t* entry, int32_t entry0, double* moments, void* stream);
+int dbir_gn_merge(const double* moments, const int64_t* pixels, const int32_t* image, int32_t entries,
+                  int32_t images, int32_t reverse, float eps, float* stats, void* stream);
 /* imgs_per_group / rows_per_group > 0: stacked twin problems (see dbir_gemm_args.groups) -- image n /
  * row r takes gamma / beta at offset (n / imgs_per_group) * C resp. (r / rows_per_group) * c. 0 = one set. */
 
