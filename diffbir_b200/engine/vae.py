@@ -8,9 +8,15 @@ fp32 NHWC residual stream; GroupNorm(eps 1e-6)+SiLU is applied while producing t
 operand of each implicit-GEMM convolution; the mid attention (head_dim = C = 512, outside the
 64-wide flash kernel) runs as S = Q K^T (GEMM) -> row softmax -> P V^T (GEMM), with V^T
 produced directly by a transposed GEMM so that every operand stays K-major.
+
+This file states the network once, for the un-tiled and the tiled engine: `VaeWalk` runs a batch through
+the encoder or the decoder as a generator that stops at each GroupNorm and asks its driver for the
+statistics. `VaeEngine` answers at once with the batch's own statistics, inside one CUDA graph per input
+shape; `vae_tiled.TiledVae` merges the statistics of all tiles of an image before any of them goes on.
 """
 from __future__ import annotations
 
+import itertools
 from typing import Dict
 
 import torch
@@ -33,7 +39,6 @@ class VaeEngine:
         self.graphs = GraphCache(self.ws)       # decode / encode replayed as one graph per input shape
         self.op_dtype = lib.operand_dtype()
         self.w: Dict[str, torch.Tensor] = {}
-        self._part = {}                          # fp32 activation data_ptr -> (GN partial-sum buffer, slots)
         w, dev = self.w, self.dev
         for k, v in sd.items():
             if k not in shapes:
@@ -59,89 +64,7 @@ class VaeEngine:
         w["quant_conv.weight"] = f32(sd["quant_conv.weight"].reshape(sd["quant_conv.weight"].shape[0], -1), dev)
         w["post_quant_conv.weight"] = f32(sd["post_quant_conv.weight"].reshape(sd["post_quant_conv.weight"].shape[0], -1), dev)
 
-    # ------------------------------------------------------------------ blocks
-    def _gn(self, x, c, nb, h, w, gamma, beta, out16, silu, out_raw=None):
-        """GroupNorm(eps 1e-6)(+SiLU) -> 16-bit operand. Statistics come from the partial sums the
-        producing conv's epilogue emitted (dbir_gemm gn_partials -> dbir_gn_finalize: no second read of
-        the fp32 tensor); tensors written by other kernels take the stand-alone statistics pass."""
-        ws = self.ws
-        stats = ws.get("gn_stats", (nb * 64,), torch.float32)
-        part = self._part.get(x.data_ptr())
-        if part is not None:
-            lib.gn_finalize(part[0], part[1], c, None, 0, 0, nb, h * w, 1e-6, stats)
-        else:
-            wsp = ws.get("gn_ws", (lib.gn_workspace_floats(nb, h * w, c),), torch.float32, zero=True)
-            lib.gn_stats(x, None, c, 0, nb, h * w, 1e-6, stats, wsp)
-        lib.gn_apply(x, None, c, 0, nb, h, w, stats, gamma, beta, out16, norm=True, silu=silu, out_raw=out_raw)
-
-    def _stats_kw(self, out: torch.Tensor, nb: int, n_cols: int, h: int, w: int) -> dict:
-        """kwargs that make a conv-mode dbir_gemm emit GroupNorm partial sums for its output `out`."""
-        slots = lib.gemm_gn_slots(h, w)
-        if slots <= 0:
-            self._part.pop(out.data_ptr(), None)
-            return {}
-        buf = self.ws.get(f"part:{out.data_ptr()}", (nb * slots * n_cols * 2,), torch.float32)
-        self._part[out.data_ptr()] = (buf, slots)
-        return dict(gn_partials=buf)
-
-    def _res(self, p, x, cin, cout, nb, h, w, out):
-        """ResnetBlock.forward (temb None) — vae.py:97-117."""
-        ws, W, M = self.ws, self.w, nb * h * w
-        a16 = ws.get("a16", (M, cin), self.op_dtype)
-        raw = ws.get("raw16", (M, cin), self.op_dtype) if cin != cout else None
-        self._gn(x, cin, nb, h, w, W[p + "norm1.weight"], W[p + "norm1.bias"], a16, True, raw)
-        h1 = ws.get("h1", (M, cout), torch.float32)
-        lib.gemm(a16, W[p + "conv1.weight"], h1, M=M, N=cout, K=9 * cin, bias=W[p + "conv1.bias"],
-                 conv=(nb, h, w, cin, 3), **self._stats_kw(h1, nb, cout, h, w))
-        b16 = ws.get("b16", (M, cout), self.op_dtype)
-        self._gn(h1, cout, nb, h, w, W[p + "norm2.weight"], W[p + "norm2.bias"], b16, True)
-        if cin != cout:
-            sk = ws.get("skip", (M, cout), torch.float32)
-            lib.gemm(raw, W[p + "nin_shortcut.weight"], sk, M=M, N=cout, K=cin, bias=W[p + "nin_shortcut.bias"])
-            res = sk
-        else:
-            res = x
-        lib.gemm(b16, W[p + "conv2.weight"], out, M=M, N=cout, K=9 * cout, bias=W[p + "conv2.bias"],
-                 residual=res, conv=(nb, h, w, cout, 3), **self._stats_kw(out, nb, cout, h, w))
-
-    def release_buffers(self) -> None:
-        """Frees the workspace and the captured encode / decode graphs; the next call re-creates them."""
-        self.ws.clear()                          # also drops the graphs (GraphCache hooks on_grow)
-        self._part.clear()
-
-    @staticmethod
-    def attn_rows(hw: int) -> int:
-        """Query rows per chunk of the mid attention's materialised S: 8192 up to 65536 tokens (2048^2 images),
-        beyond that a multiple of 128 that keeps the fp32 S at or below 2 GiB (3584 rows at 3072^2)."""
-        return min(8192, max(128, (2 ** 31 // (4 * hw)) // 128 * 128))
-
-    def _attn(self, p, x, c, nb, h, w):
-        """Single-head attention over pixels, in place on x — vae.py:232-282."""
-        ws, W, hw = self.ws, self.w, h * w
-        M = nb * hw
-        a16 = ws.get("a16", (M, c), self.op_dtype)
-        self._gn(x, c, nb, h, w, W[p + "norm.weight"], W[p + "norm.bias"], a16, False)
-        qk = ws.get("qk16", (M, 2 * c), self.op_dtype)
-        lib.gemm(a16, W[p + "qk.w"], qk, M=M, N=2 * c, K=c, bias=W[p + "qk.b"])
-        o16 = ws.get("o16", (M, c), self.op_dtype)
-        rows = min(hw, self.attn_rows(hw))
-        for b in range(nb):
-            a_b = a16[b * hw:(b + 1) * hw]
-            vt = ws.get("vt16", (c, hw), self.op_dtype)               # V^T [C, hw]
-            lib.gemm(W[p + "v.weight"], a_b, vt, M=c, N=hw, K=c, bias=W[p + "v.bias"], bias_per_row=True)
-            for r0 in range(0, hw, rows):
-                r1 = min(hw, r0 + rows)
-                s = ws.get("s32", (r1 - r0, hw), torch.float32)
-                qb = qk[b * hw + r0: b * hw + r1]
-                kb = qk[b * hw:(b + 1) * hw, c:]
-                lib.gemm(qb, kb, s, M=r1 - r0, N=hw, K=c, lda=2 * c, ldb=2 * c)
-                p16 = ws.get("p16", (r1 - r0, hw), self.op_dtype)
-                lib.softmax_rows(s, hw, r1 - r0, hw, float(c) ** -0.5, p16, hw)
-                lib.gemm(p16, vt, o16[b * hw + r0: b * hw + r1], M=r1 - r0, N=c, K=hw)
-        lib.gemm(o16, W[p + "proj_out.weight"], x, M=M, N=c, K=c, bias=W[p + "proj_out.bias"], residual=x)
-        self._part.pop(x.data_ptr(), None)                       # x changed in place: its partials are stale
-
-    # ------------------------------------------------------------------ decode
+    # ------------------------------------------------------------------ un-tiled driver
     def decode(self, z: torch.Tensor) -> torch.Tensor:
         """z fp32 NCHW [nb, 4, h, w] (already divided by the scale factor) -> image fp32 NCHW
         [nb, 3, 8h, 8w] in [-1, 1]."""
@@ -149,93 +72,255 @@ class VaeEngine:
         return self.graphs.run(("dec",) + tuple(z.shape), self._decode, z)
 
     def _decode(self, z: torch.Tensor) -> torch.Tensor:
-        cfg, ws, W = self.cfg, self.ws, self.w
-        nb, zc, h, w = z.shape
-        ch, mult, nres = cfg["ch"], tuple(cfg["ch_mult"]), cfg["num_res_blocks"]
-        # post_quant_conv (1x1, 4->4) on NHWC rows, fp32
-        z_nhwc = ws.get("z_nhwc", (nb * h * w, zc), torch.float32)
-        lib.nchw_to_nhwc(z, nb, zc, h * w, z_nhwc)
-        z2 = ws.get("z2", (nb * h * w, zc), torch.float32)
-        lib.linear_f32(z_nhwc, zc, nb * h * w, zc, W["post_quant_conv.weight"], W["post_quant_conv.bias"], zc, z2, zc)
-        z2n = ws.get("z2n", (nb, zc, h, w), torch.float32)
-        lib.nhwc_to_nchw(z2, nb, zc, h * w, z2n)
-        p = "decoder."
-        c = ch * mult[-1]
-        x = ws.get("x0", (nb * h * w, c), torch.float32)
-        lib.conv3x3_small_cin(z2n, None, zc, 0, nb, h, w, W[p + "conv_in.weight"], W[p + "conv_in.bias"], c, x)
-        self._part.pop(x.data_ptr(), None)                       # written without GEMM partials
-        self._res(p + "mid.block_1.", x, c, c, nb, h, w, x)
-        self._attn(p + "mid.attn_1.", x, c, nb, h, w)
-        self._res(p + "mid.block_2.", x, c, c, nb, h, w, x)
-        cur, flip = x, 0
-        for lvl in reversed(range(len(mult))):
-            cout = ch * mult[lvl]
-            for j in range(nres + 1):
-                o = ws.get(f"x{1 + flip}", (nb * h * w, cout), torch.float32)
-                self._res(f"{p}up.{lvl}.block.{j}.", cur, c, cout, nb, h, w, o)
-                cur, c, flip = o, cout, flip ^ 1
-            if lvl != 0:
-                up16 = ws.get("a16", (nb * 4 * h * w, c), self.op_dtype)
-                lib.gn_apply(cur, None, c, 0, nb, h, w, None, None, None, up16, norm=False, silu=False, upsample=2)
-                o = ws.get(f"x{1 + flip}", (nb * 4 * h * w, c), torch.float32)
-                lib.gemm(up16, W[f"{p}up.{lvl}.upsample.conv.weight"], o, M=nb * 4 * h * w, N=c, K=9 * c,
-                         bias=W[f"{p}up.{lvl}.upsample.conv.bias"], conv=(nb, 2 * h, 2 * w, c, 3),
-                         **self._stats_kw(o, nb, c, 2 * h, 2 * w))
-                cur, flip, h, w = o, flip ^ 1, 2 * h, 2 * w
-        a16 = ws.get("a16", (nb * h * w, c), self.op_dtype)
-        self._gn(cur, c, nb, h, w, W[p + "norm_out.weight"], W[p + "norm_out.bias"], a16, True)
-        out = torch.empty(nb, cfg["out_ch"], h, w, dtype=torch.float32, device=self.dev)
-        lib.conv3x3_small_cout(a16, nb, h, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"],
-                               cfg["out_ch"], out, nchw=True)
-        return out
+        return self._drive(VaeWalk.decoder, self.post_quant(z, self._scratch()))
 
-    # ------------------------------------------------------------------ encode
     def encode_moments(self, img: torch.Tensor) -> torch.Tensor:
         """img fp32 NCHW [nb, 3, H, W] in [-1, 1] -> moments fp32 NCHW [nb, 8, H/8, W/8]."""
         assert img.is_cuda and img.dtype == torch.float32 and img.is_contiguous()
         return self.graphs.run(("enc",) + tuple(img.shape), self._encode_moments, img)
 
     def _encode_moments(self, img: torch.Tensor) -> torch.Tensor:
-        cfg, ws, W = self.cfg, self.ws, self.w
-        nb, ic, h, w = img.shape
-        ch, mult, nres = cfg["ch"], tuple(cfg["ch_mult"]), cfg["num_res_blocks"]
-        p = "encoder."
-        c = ch
-        cur = ws.get("x0", (nb * h * w, c), torch.float32)
-        lib.conv3x3_small_cin(img, None, ic, 0, nb, h, w, W[p + "conv_in.weight"], W[p + "conv_in.bias"], c, cur)
-        self._part.pop(cur.data_ptr(), None)                     # written without GEMM partials
-        flip = 0
-        for lvl in range(len(mult)):
-            cout = ch * mult[lvl]
-            for j in range(nres):
-                o = ws.get(f"x{1 + flip}", (nb * h * w, cout), torch.float32)
-                self._res(f"{p}down.{lvl}.block.{j}.", cur, c, cout, nb, h, w, o)
-                cur, c, flip = o, cout, flip ^ 1
-            if lvl != len(mult) - 1:
-                ho, wo = h // 2, w // 2
-                col = ws.get("a16", (nb * ho * wo, 9 * c), self.op_dtype)
-                lib.im2col_s2(cur, nb, h, w, c, 0, col)
-                o = ws.get(f"x{1 + flip}", (nb * ho * wo, c), torch.float32)
-                lib.gemm(col, W[f"{p}down.{lvl}.downsample.conv.weight"], o, M=nb * ho * wo, N=c, K=9 * c,
-                         bias=W[f"{p}down.{lvl}.downsample.conv.bias"])
-                self._part.pop(o.data_ptr(), None)               # plain-mode GEMM: no partials requested
-                cur, flip, h, w = o, flip ^ 1, ho, wo
-        self._res(p + "mid.block_1.", cur, c, c, nb, h, w, cur)
-        self._attn(p + "mid.attn_1.", cur, c, nb, h, w)
-        self._res(p + "mid.block_2.", cur, c, c, nb, h, w, cur)
-        a16 = ws.get("a16", (nb * h * w, c), self.op_dtype)
-        self._gn(cur, c, nb, h, w, W[p + "norm_out.weight"], W[p + "norm_out.bias"], a16, True)
-        zc2 = 2 * cfg["z_channels"]
-        m_nhwc = ws.get("m_nhwc", (nb * h * w, zc2), torch.float32)
-        lib.conv3x3_small_cout(a16, nb, h, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], zc2,
-                               m_nhwc, nchw=False)
-        q = ws.get("q_nhwc", (nb * h * w, zc2), torch.float32)
-        lib.linear_f32(m_nhwc, zc2, nb * h * w, zc2, W["quant_conv.weight"], W["quant_conv.bias"], zc2, q, zc2)
-        out = torch.empty(nb, zc2, h, w, dtype=torch.float32, device=self.dev)
-        lib.nhwc_to_nchw(q, nb, zc2, h * w, out)
-        return out
+        return self.quant(self._drive(VaeWalk.encoder, img), self._scratch())
 
     def encode_mode(self, img: torch.Tensor, scale_factor: float = 0.18215) -> torch.Tensor:
         """ControlLDM.vae_encode(sample=False) — cldm.py:92-119: posterior mean * scale."""
         m = self.encode_moments(img)
         return (m[:, : m.shape[1] // 2] * scale_factor).contiguous()
+
+    def _drive(self, net, x: torch.Tensor) -> torch.Tensor:
+        """Runs the batch x through `net` (VaeWalk.encoder / .decoder), answering each GroupNorm at once with the
+        batch's own statistics: from the partial sums the producing conv's epilogue emitted (dbir_gemm gn_partials
+        -> dbir_gn_finalize: no second read of the fp32 tensor); tensors written by other kernels take the
+        stand-alone statistics pass.
+
+        The walk's fp32 activations come from three workspace buffers, so nothing is allocated during graph
+        capture. A buffer is handed out again once the tensor it last held has left the walk's state. Three are
+        enough: the walk allocates only while st holds at most two tensors (a ResnetBlock keeps its input or its
+        shortcut, and conv1's output while conv2's is allocated), and it reads a tensor that has left the state
+        only in launches issued before its next allocation. These three are all the full-resolution fp32
+        memory of the un-tiled VAE, which is what bounds the largest image that runs without tiling."""
+        ws, nb = self.ws, x.shape[0]
+        st: Dict[str, torch.Tensor] = {}
+        held = [None] * 3
+
+        def new(*shape):
+            i = next(i for i, t in enumerate(held) if not any(t is v for v in st.values()))
+            held[i] = ws.get(f"x{i}", shape, torch.float32)
+            return held[i]
+
+        gen = net(VaeWalk(self, st, new, ws, nb), x)
+        stats, answer = ws.get("gn_stats", (nb * 64,), torch.float32), None
+        try:
+            while True:
+                c, h, w, part, slots = gen.send(answer)
+                if part is not None:
+                    lib.gn_finalize(part, slots, c, None, 0, 0, nb, h * w, 1e-6, stats)
+                else:
+                    wsp = ws.get("gn_ws", (lib.gn_workspace_floats(nb, h * w, c),), torch.float32, zero=True)
+                    lib.gn_stats(st["cur"], None, c, 0, nb, h * w, 1e-6, stats, wsp)
+                answer = stats
+        except StopIteration as end:
+            return end.value
+
+    def _scratch(self):
+        """Allocator for the quant convs inside the graph: each call hands out a workspace buffer of its own."""
+        n = itertools.count()
+        return lambda *shape: self.ws.get(f"q{next(n)}", shape, torch.float32)
+
+    def release_buffers(self) -> None:
+        """Frees the workspace and the captured encode / decode graphs; the next call re-creates them."""
+        self.ws.clear()                          # also drops the graphs (GraphCache hooks on_grow)
+
+    # ------------------------------------------------------------------ the ends (un-tiled in both engines)
+    def post_quant(self, z: torch.Tensor, new) -> torch.Tensor:
+        """post_quant_conv (1x1, 4->4) on NHWC rows, fp32: z NCHW -> the decoder's input, NCHW. new(*shape)
+        supplies the fp32 tensors."""
+        nb, zc, h, w = z.shape
+        z_nhwc = new(nb * h * w, zc)
+        lib.nchw_to_nhwc(z, nb, zc, h * w, z_nhwc)
+        z2 = new(nb * h * w, zc)
+        lib.linear_f32(z_nhwc, zc, nb * h * w, zc, self.w["post_quant_conv.weight"], self.w["post_quant_conv.bias"],
+                       zc, z2, zc)
+        out = new(nb, zc, h, w)
+        lib.nhwc_to_nchw(z2, nb, zc, h * w, out)
+        return out
+
+    def quant(self, m: torch.Tensor, new) -> torch.Tensor:
+        """quant_conv (1x1, 8->8) on the encoder's output m, fp32 NHWC [nb, h, w, 8] -> moments NCHW."""
+        nb, h, w, zc2 = m.shape
+        q = new(nb * h * w, zc2)
+        lib.linear_f32(m, zc2, nb * h * w, zc2, self.w["quant_conv.weight"], self.w["quant_conv.bias"], zc2, q, zc2)
+        out = torch.empty(nb, zc2, h, w, dtype=torch.float32, device=self.dev)
+        lib.nhwc_to_nchw(q, nb, zc2, h * w, out)
+        return out
+
+    @staticmethod
+    def attn_rows(hw: int) -> int:
+        """Query rows per chunk of the mid attention's materialised S: 8192 up to 65536 tokens (2048^2 images),
+        beyond that a multiple of 128 that keeps the fp32 S at or below 2 GiB (3584 rows at 3072^2)."""
+        return min(8192, max(128, (2 ** 31 // (4 * hw)) // 128 * 128))
+
+
+NO_PARTIALS = (None, 0)
+
+
+class VaeWalk:
+    """One batch of nb images (or tiles) through the encoder or the decoder of `eng`, as generators that stop at
+    each GroupNorm: 22 times in the encoder, 30 in the decoder.
+
+    At a GroupNorm the walk yields (c, h, w, partials, slots): st["cur"], fp32 NHWC [nb * h * w, c], is about
+    to be normalised, and `partials` are the GroupNorm partial sums (`slots` per image) that the convolution
+    which wrote it emitted, or None where another kernel wrote it. The driver sends back the fp32 [nb * 64]
+    (mean, rstd) buffer that dbir_gn_apply reads. A convolution's partial sums are read at the next yield and
+    nowhere else, so one workspace buffer holds them all.
+
+    The driver supplies the state `st` (the fp32 activations that live from one GroupNorm to the next: "cur" and,
+    inside a ResnetBlock, the pending residual "res"), new(*shape) for fresh fp32 tensors, and the workspace for
+    the 16-bit operands and scratch. No fp32 activation is held in a local across a yield, and none is read after
+    it has left st and new() was called again: between yields a driver may move the state elsewhere, and new()
+    may hand out the memory of a tensor that is no longer in st. Split-K is off in every GEMM, so an image's bits
+    do not depend on the batch it runs in."""
+
+    def __init__(self, eng: VaeEngine, st: Dict[str, torch.Tensor], new, ws: Workspace, nb: int):
+        self.w, self.cfg, self.dev, self.op_dtype = eng.w, eng.cfg, eng.dev, eng.op_dtype
+        self.st, self.new, self.ws, self.nb = st, new, ws, nb
+
+    def _conv(self, a16, key, out, cin, cout, h, w, residual=None, partials=True):
+        """3x3 implicit-GEMM convolution into `out`. Returns the (partials, slots) to yield at the GroupNorm of
+        `out`: NO_PARTIALS when they are not asked for (`out` feeds a resampling, not a GroupNorm) or the GEMM
+        cannot emit them for this image shape."""
+        W, nb = self.w, self.nb
+        slots = lib.gemm_gn_slots(h, w) if partials else 0
+        part = self.ws.get("part", (nb * slots * cout * 2,), torch.float32) if slots > 0 else None
+        lib.gemm(a16, W[key + ".weight"], out, M=nb * h * w, N=cout, K=9 * cin, bias=W[key + ".bias"],
+                 residual=residual, conv=(nb, h, w, cin, 3), split_k=1, gn_partials=part)
+        return (part, slots) if slots > 0 else NO_PARTIALS
+
+    def _res(self, p, cin, cout, h, w, src, partials=True):
+        """ResnetBlock.forward (temb None) — vae.py:97-117 — on st["cur"], whose partial sums are `src`; returns
+        those of its output."""
+        ws, W, st, nb, M = self.ws, self.w, self.st, self.nb, self.nb * h * w
+        stats = yield (cin, h, w) + src
+        a16 = ws.get("a16", (M, cin), self.op_dtype)
+        raw = ws.get("raw16", (M, cin), self.op_dtype) if cin != cout else None
+        lib.gn_apply(st["cur"], None, cin, 0, nb, h, w, stats, W[p + "norm1.weight"], W[p + "norm1.bias"], a16,
+                     norm=True, silu=True, out_raw=raw)
+        if cin != cout:
+            st["res"] = self.new(M, cout)
+            lib.gemm(raw, W[p + "nin_shortcut.weight"], st["res"], M=M, N=cout, K=cin, bias=W[p + "nin_shortcut.bias"],
+                     split_k=1)
+            del st["cur"]
+        else:
+            st["res"] = st.pop("cur")
+        st["cur"] = self.new(M, cout)
+        src = self._conv(a16, p + "conv1", st["cur"], cin, cout, h, w)
+        stats = yield (cout, h, w) + src
+        b16 = ws.get("b16", (M, cout), self.op_dtype)
+        lib.gn_apply(st["cur"], None, cout, 0, nb, h, w, stats, W[p + "norm2.weight"], W[p + "norm2.bias"], b16,
+                     norm=True, silu=True)
+        st["cur"] = self.new(M, cout)
+        return self._conv(b16, p + "conv2", st["cur"], cout, cout, h, w, residual=st.pop("res"), partials=partials)
+
+    def _attn(self, p, c, h, w, src):
+        """AttnBlock (single head over the pixels of each image) — vae.py:232-282 — in place on st["cur"]."""
+        ws, W, nb, hw = self.ws, self.w, self.nb, h * w
+        M = nb * hw
+        stats = yield (c, h, w) + src
+        x = self.st["cur"]
+        a16 = ws.get("a16", (M, c), self.op_dtype)
+        lib.gn_apply(x, None, c, 0, nb, h, w, stats, W[p + "norm.weight"], W[p + "norm.bias"], a16, norm=True,
+                     silu=False)
+        qk = ws.get("qk16", (M, 2 * c), self.op_dtype)
+        lib.gemm(a16, W[p + "qk.w"], qk, M=M, N=2 * c, K=c, bias=W[p + "qk.b"], split_k=1)
+        o16 = ws.get("o16", (M, c), self.op_dtype)
+        rows = min(hw, VaeEngine.attn_rows(hw))
+        # any token count: the key axis of S, P and V^T is padded to a multiple of 8 (16-byte GEMM rows); the
+        # softmax runs over the real keys and the padded columns of P and V^T are zero
+        kp = -(-hw // 8) * 8
+        vt = ws.get("vt16", (c, kp), self.op_dtype)                    # V^T [C, keys]
+        p16 = ws.get("p16", (rows, kp), self.op_dtype)
+        vt[:, hw:].zero_()
+        p16[:, hw:].zero_()
+        for b in range(nb):
+            lib.gemm(W[p + "v.weight"], a16[b * hw:(b + 1) * hw], vt, M=c, N=hw, K=c, bias=W[p + "v.bias"],
+                     bias_per_row=True, ldo=kp, split_k=1)
+            for r0 in range(0, hw, rows):
+                r1 = min(hw, r0 + rows)
+                s = ws.get("s32", (r1 - r0, kp), torch.float32)
+                lib.gemm(qk[b * hw + r0: b * hw + r1], qk[b * hw:(b + 1) * hw, c:], s, M=r1 - r0, N=hw, K=c,
+                         lda=2 * c, ldb=2 * c, ldo=kp, split_k=1)
+                lib.softmax_rows(s, kp, r1 - r0, hw, float(c) ** -0.5, p16, kp)
+                lib.gemm(p16[:r1 - r0], vt, o16[b * hw + r0: b * hw + r1], M=r1 - r0, N=c, K=kp, split_k=1)
+        lib.gemm(o16, W[p + "proj_out.weight"], x, M=M, N=c, K=c, bias=W[p + "proj_out.bias"], residual=x, split_k=1)
+        return NO_PARTIALS
+
+    def _mid(self, p, c, h, w, src):
+        src = yield from self._res(p + "mid.block_1.", c, c, h, w, src)
+        src = yield from self._attn(p + "mid.attn_1.", c, h, w, src)
+        return (yield from self._res(p + "mid.block_2.", c, c, h, w, src))
+
+    def encoder(self, img: torch.Tensor):
+        """img fp32 NCHW [nb, 3, h, w] -> the encoder's output before quant_conv, fp32 NHWC [nb, h/8, w/8, 8]."""
+        cfg, ws, W, st, nb = self.cfg, self.ws, self.w, self.st, self.nb
+        ch, mult, nres = cfg["ch"], tuple(cfg["ch_mult"]), cfg["num_res_blocks"]
+        _, ic, h, w = img.shape
+        p, c = "encoder.", ch
+        st["cur"] = self.new(nb * h * w, c)
+        lib.conv3x3_small_cin(img, None, ic, 0, nb, h, w, W[p + "conv_in.weight"], W[p + "conv_in.bias"], c, st["cur"])
+        del img
+        src = NO_PARTIALS
+        for lvl in range(len(mult)):
+            cout = ch * mult[lvl]
+            down = lvl != len(mult) - 1
+            for j in range(nres):
+                src = yield from self._res(f"{p}down.{lvl}.block.{j}.", c, cout, h, w, src,
+                                           partials=not (down and j == nres - 1))
+                c = cout
+            if down:
+                ho, wo = h // 2, w // 2
+                col = ws.get("a16", (nb * ho * wo, 9 * c), self.op_dtype)
+                lib.im2col_s2(st["cur"], nb, h, w, c, 0, col)
+                st["cur"] = self.new(nb * ho * wo, c)
+                lib.gemm(col, W[f"{p}down.{lvl}.downsample.conv.weight"], st["cur"], M=nb * ho * wo, N=c, K=9 * c,
+                         bias=W[f"{p}down.{lvl}.downsample.conv.bias"], split_k=1)
+                h, w, src = ho, wo, NO_PARTIALS                   # a plain-mode GEMM emits none
+        src = yield from self._mid(p, c, h, w, src)
+        stats = yield (c, h, w) + src
+        a16 = ws.get("a16", (nb * h * w, c), self.op_dtype)
+        lib.gn_apply(st.pop("cur"), None, c, 0, nb, h, w, stats, W[p + "norm_out.weight"], W[p + "norm_out.bias"],
+                     a16, norm=True, silu=True)
+        zc2 = 2 * cfg["z_channels"]
+        m = self.new(nb, h, w, zc2)
+        lib.conv3x3_small_cout(a16, nb, h, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], zc2, m, nchw=False)
+        return m
+
+    def decoder(self, z: torch.Tensor):
+        """z fp32 NCHW [nb, 4, h, w], after post_quant_conv -> image fp32 NCHW [nb, 3, 8h, 8w], a tensor of its own."""
+        cfg, ws, W, st, nb = self.cfg, self.ws, self.w, self.st, self.nb
+        ch, mult, nres = cfg["ch"], tuple(cfg["ch_mult"]), cfg["num_res_blocks"]
+        _, zc, h, w = z.shape
+        p, c = "decoder.", ch * mult[-1]
+        st["cur"] = self.new(nb * h * w, c)
+        lib.conv3x3_small_cin(z, None, zc, 0, nb, h, w, W[p + "conv_in.weight"], W[p + "conv_in.bias"], c, st["cur"])
+        del z
+        src = yield from self._mid(p, c, h, w, NO_PARTIALS)
+        for lvl in reversed(range(len(mult))):
+            cout = ch * mult[lvl]
+            for j in range(nres + 1):
+                src = yield from self._res(f"{p}up.{lvl}.block.{j}.", c, cout, h, w, src,
+                                           partials=not (lvl != 0 and j == nres))
+                c = cout
+            if lvl != 0:
+                up16 = ws.get("a16", (nb * 4 * h * w, c), self.op_dtype)
+                lib.gn_apply(st["cur"], None, c, 0, nb, h, w, None, None, None, up16, norm=False, silu=False, upsample=2)
+                h, w = 2 * h, 2 * w
+                st["cur"] = self.new(nb * h * w, c)
+                src = self._conv(up16, f"{p}up.{lvl}.upsample.conv", st["cur"], c, c, h, w)
+        stats = yield (c, h, w) + src
+        a16 = ws.get("a16", (nb * h * w, c), self.op_dtype)
+        lib.gn_apply(st.pop("cur"), None, c, 0, nb, h, w, stats, W[p + "norm_out.weight"], W[p + "norm_out.bias"],
+                     a16, norm=True, silu=True)
+        out = torch.empty(nb, cfg["out_ch"], h, w, dtype=torch.float32, device=self.dev)
+        lib.conv3x3_small_cout(a16, nb, h, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], cfg["out_ch"], out,
+                               nchw=True)
+        return out

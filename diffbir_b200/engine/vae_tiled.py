@@ -12,11 +12,13 @@ Semantics (these are the reference's, not the un-tiled VAE's):
 * quant_conv / post_quant_conv run un-tiled.
 
 Execution: tiles of equal shape form a shape class; a class runs as batched "waves" of whole tiles (all images
-of a tile together) through the same kernels as VaeEngine, with split-K off so that a tile's bits do not depend
-on its wave. The network is cut at each GroupNorm into segments: every wave runs a segment and emits its moments,
-the moments are merged, then the next segment starts. Between segments a wave carries its state (the current
-fp32 tensor and the pending residual); beyond `state_budget` bytes the state is staged through pinned host
-buffers on a side stream, overlapped with the next wave. Launches are eager (no CUDA graphs).
+of a tile together). The network itself is stated in vae.py: each wave runs `VaeWalk`, the generator VaeEngine
+runs too (same kernels, split-K off so that a tile's bits do not depend on its wave), which stops at each
+GroupNorm. This file supplies what is the tiled engine's own: the tile plan, the waves, and the driver (`_run`)
+that at each stop takes every wave's moments, merges them and sends the statistics back. Between stops a wave
+carries its state (the current fp32 tensor and the pending residual, fresh `torch.empty` tensors in the wave's
+`st`); beyond `state_budget` bytes the state is staged through pinned host buffers on a side stream, overlapped
+with the next wave. Launches are eager (no CUDA graphs).
 """
 from __future__ import annotations
 
@@ -28,7 +30,7 @@ import torch
 
 from .. import lib
 from .common import Workspace
-from .vae import VaeEngine
+from .vae import VaeEngine, VaeWalk
 
 PAD_ENCODER = 32        # image pixels
 PAD_DECODER = 11        # latent pixels
@@ -125,8 +127,7 @@ class TiledVae:
     wave_pixels: int = 1 << 22
 
     def __init__(self, base: VaeEngine):
-        self.base, self.w, self.cfg, self.dev = base, base.w, base.cfg, base.dev
-        self.op_dtype = base.op_dtype
+        self.base, self.cfg, self.dev = base, base.cfg, base.dev
         self.ws = Workspace(self.dev)
         self.last_stats: dict = {}
 
@@ -144,13 +145,8 @@ class TiledVae:
             plan = plan_vae_tiles(h, w, tile_size, False)
         zc2 = 2 * self.cfg["z_channels"]
         res = torch.empty(n, h // 8, w // 8, zc2, dtype=torch.float32, device=self.dev)      # NHWC
-        self._run(plan, img, res, self._encoder, 1)
-        rows = n * (h // 8) * (w // 8)
-        q = torch.empty(rows, zc2, dtype=torch.float32, device=self.dev)
-        lib.linear_f32(res, zc2, rows, zc2, self.w["quant_conv.weight"], self.w["quant_conv.bias"], zc2, q, zc2)
-        out = torch.empty(n, zc2, h // 8, w // 8, dtype=torch.float32, device=self.dev)
-        lib.nhwc_to_nchw(q, n, zc2, (h // 8) * (w // 8), out)
-        return out
+        self._run(plan, img, res, False)
+        return self.base.quant(res, self._new)
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor, tile_size: int) -> torch.Tensor:
@@ -164,16 +160,9 @@ class TiledVae:
             plan = whole_image_plan(h, w, True)
         else:
             plan = plan_vae_tiles(h, w, tile_size, True)
-        z_nhwc = torch.empty(n * h * w, zc, dtype=torch.float32, device=self.dev)
-        lib.nchw_to_nhwc(z, n, zc, h * w, z_nhwc)
-        z2 = torch.empty_like(z_nhwc)
-        lib.linear_f32(z_nhwc, zc, n * h * w, zc, self.w["post_quant_conv.weight"], self.w["post_quant_conv.bias"],
-                       zc, z2, zc)
-        z2n = torch.empty(n, zc, h, w, dtype=torch.float32, device=self.dev)
-        lib.nhwc_to_nchw(z2, n, zc, h * w, z2n)
-        del z_nhwc, z2
+        z2n = self.base.post_quant(z, self._new)
         res = torch.empty(n, self.cfg["out_ch"], 8 * h, 8 * w, dtype=torch.float32, device=self.dev)
-        self._run(plan, z2n, res, self._decoder, 8)
+        self._run(plan, z2n, res, True)
         return res
 
     def release_buffers(self) -> None:
@@ -189,9 +178,9 @@ class TiledVae:
                 waves.append(_Wave(tiles[i:i + per], n_img, shape, self.dev))
         return waves
 
-    def _run(self, plan: TilePlan, src: torch.Tensor, res: torch.Tensor, net, up: int) -> None:
+    def _run(self, plan: TilePlan, src: torch.Tensor, res: torch.Tensor, decoder: bool) -> None:
         n_img = src.shape[0]
-        waves = self._waves(plan, n_img, up)
+        waves = self._waves(plan, n_img, 8 if decoder else 1)
         entries = len(plan.in_boxes) * n_img
         self._moments = torch.empty(entries, 32, 2, dtype=torch.float64, device=self.dev)
         stats = torch.empty(entries, 64, dtype=torch.float32, device=self.dev)
@@ -203,7 +192,7 @@ class TiledVae:
         main = torch.cuda.current_stream(self.dev)
         self._side = torch.cuda.Stream(self.dev)
         for wv in waves:
-            wv.gen = net(wv, plan, src, res)
+            wv.gen = self._tiles(wv, plan, src, res, decoder)
         passes, spills = 0, 0
         try:
             sent: List[Optional[torch.Tensor]] = [None] * len(waves)
@@ -214,10 +203,12 @@ class TiledVae:
                     if i + 1 < len(waves):
                         self._prefetch(waves[i + 1])
                     try:
-                        pix.append(wv.gen.send(sent[i]) if passes else next(wv.gen))
+                        c, h, w, part, slots = wv.gen.send(sent[i]) if passes else next(wv.gen)
                     except StopIteration:
                         done += 1
                         continue
+                    self._emit(wv, c, h, w, part, slots)
+                    pix.append(h * w)
                     size = sum(t.numel() * t.element_size() for t in wv.st.values())
                     if kept + size <= budget:
                         kept += size
@@ -293,172 +284,32 @@ class TiledVae:
                 t.record_stream(main)
             wv.loaded = None
 
-    # ------------------------------------------------------------------ blocks (generators: one yield per GroupNorm)
+    # ------------------------------------------------------------------ one wave through the network
     def _new(self, *shape) -> torch.Tensor:
         return torch.empty(*shape, dtype=torch.float32, device=self.dev)
 
-    def _emit(self, wv: _Wave, x: torch.Tensor, c: int, h: int, w: int, part=None, slots=0) -> None:
-        """Moments of the wave's fp32 NHWC tensor x into the call's moment buffer, at its entries' indices."""
+    def _emit(self, wv: _Wave, c: int, h: int, w: int, part, slots: int) -> None:
+        """Moments of the wave's st["cur"] into the call's moment buffer, at its entries' indices: from the partial
+        sums of the conv that wrote it, or, where there are none, from the tensor itself."""
         if part is not None:
             lib.gn_moments(c, wv.nb, h * w, self._moments, partials=part, slots=slots, entry=wv.entries)
         else:
             ws = self.ws.get("mom_ws", (lib.gn_moments_workspace_floats(wv.nb, h * w, c),), torch.float32)
-            lib.gn_moments(c, wv.nb, h * w, self._moments, x=x, workspace=ws, entry=wv.entries)
+            lib.gn_moments(c, wv.nb, h * w, self._moments, x=wv.st["cur"], workspace=ws, entry=wv.entries)
 
-    def _conv(self, wv, a16, key, out, cin, cout, h, w, residual=None, emit=True) -> None:
-        """3x3 implicit-GEMM convolution of the wave; emits the output's moments from the fused partial sums
-        (or, where the GEMM cannot emit them for this tile shape, from the output itself)."""
-        W = self.w
-        slots = lib.gemm_gn_slots(h, w) if emit else 0
-        part = self.ws.get("part", (wv.nb * slots * cout * 2,), torch.float32) if slots > 0 else None
-        lib.gemm(a16, W[key + ".weight"], out, M=wv.nb * h * w, N=cout, K=9 * cin, bias=W[key + ".bias"],
-                 residual=residual, conv=(wv.nb, h, w, cin, 3), split_k=1, gn_partials=part)
-        if emit:
-            self._emit(wv, out, cout, h, w, part, slots)
-
-    def _res(self, wv, p, cin, cout, h, w, emit=True):
-        """ResnetBlock (vae.py:97-117) on st["cur"]; reads its statistics at two yields. No device tensor is
-        held in a local across a yield: the state may be staged to the host in between."""
-        ws, W, st, M, nb = self.ws, self.w, wv.st, wv.nb * h * w, wv.nb
-        stats = yield h * w
-        a16 = ws.get("a16", (M, cin), self.op_dtype)
-        raw = ws.get("raw16", (M, cin), self.op_dtype) if cin != cout else None
-        lib.gn_apply(st["cur"], None, cin, 0, nb, h, w, stats, W[p + "norm1.weight"], W[p + "norm1.bias"], a16,
-                     norm=True, silu=True, out_raw=raw)
-        if cin != cout:
-            st["res"] = self._new(M, cout)
-            lib.gemm(raw, W[p + "nin_shortcut.weight"], st["res"], M=M, N=cout, K=cin, bias=W[p + "nin_shortcut.bias"],
-                     split_k=1)
-            del st["cur"]
-        else:
-            st["res"] = st.pop("cur")
-        st["cur"] = self._new(M, cout)
-        self._conv(wv, a16, p + "conv1", st["cur"], cin, cout, h, w)
-        stats = yield h * w
-        b16 = ws.get("b16", (M, cout), self.op_dtype)
-        lib.gn_apply(st["cur"], None, cout, 0, nb, h, w, stats, W[p + "norm2.weight"], W[p + "norm2.bias"], b16,
-                     norm=True, silu=True)
-        st["cur"] = self._new(M, cout)
-        self._conv(wv, b16, p + "conv2", st["cur"], cout, cout, h, w, residual=st.pop("res"), emit=emit)
-
-    def _attn(self, wv, p, c, h, w):
-        """AttnBlock (vae.py:232-282) in place on st["cur"], each entry attending over its own tile's tokens."""
-        ws, W, st, nb, hw = self.ws, self.w, wv.st, wv.nb, h * w
-        M = nb * hw
-        stats = yield hw
-        x = st["cur"]
-        a16 = ws.get("a16", (M, c), self.op_dtype)
-        lib.gn_apply(x, None, c, 0, nb, h, w, stats, W[p + "norm.weight"], W[p + "norm.bias"], a16, norm=True,
-                     silu=False)
-        qk = ws.get("qk16", (M, 2 * c), self.op_dtype)
-        lib.gemm(a16, W[p + "qk.w"], qk, M=M, N=2 * c, K=c, bias=W[p + "qk.b"], split_k=1)
-        o16 = ws.get("o16", (M, c), self.op_dtype)
-        rows = min(hw, VaeEngine.attn_rows(hw))
-        # tiles have any token count: the key axis of S, P and V^T is padded to a multiple of 8 (16-byte GEMM rows);
-        # the softmax runs over the real keys and the padded columns of P and V^T are zero
-        kp = -(-hw // 8) * 8
-        vt = ws.get("vt16", (c, kp), self.op_dtype)
-        p16 = ws.get("p16", (rows, kp), self.op_dtype)
-        vt[:, hw:].zero_()
-        p16[:, hw:].zero_()
-        for b in range(nb):
-            lib.gemm(W[p + "v.weight"], a16[b * hw:(b + 1) * hw], vt, M=c, N=hw, K=c, bias=W[p + "v.bias"],
-                     bias_per_row=True, ldo=kp, split_k=1)
-            for r0 in range(0, hw, rows):
-                r1 = min(hw, r0 + rows)
-                s = ws.get("s32", (r1 - r0, kp), torch.float32)
-                lib.gemm(qk[b * hw + r0: b * hw + r1], qk[b * hw:(b + 1) * hw, c:], s, M=r1 - r0, N=hw, K=c,
-                         lda=2 * c, ldb=2 * c, ldo=kp, split_k=1)
-                lib.softmax_rows(s, kp, r1 - r0, hw, float(c) ** -0.5, p16, kp)
-                lib.gemm(p16[:r1 - r0], vt, o16[b * hw + r0: b * hw + r1], M=r1 - r0, N=c, K=kp, split_k=1)
-        lib.gemm(o16, W[p + "proj_out.weight"], x, M=M, N=c, K=c, bias=W[p + "proj_out.bias"], residual=x, split_k=1)
-        self._emit(wv, x, c, h, w)
-        del x
-
-    def _mid(self, wv, p, c, h, w):
-        yield from self._res(wv, p + "mid.block_1.", c, c, h, w)
-        yield from self._attn(wv, p + "mid.attn_1.", c, h, w)
-        yield from self._res(wv, p + "mid.block_2.", c, c, h, w)
-
-    def _gather(self, wv: _Wave, plan: TilePlan, src: torch.Tensor) -> torch.Tensor:
-        """The wave's input tiles as one NCHW batch, tile-major (entry = tile * N + image)."""
-        parts = []
-        for t in wv.tiles:
-            x0, x1, y0, y1 = plan.in_boxes[t]
-            parts.append(src[:, :, y0:y1, x0:x1])
-        return torch.cat(parts, 0).contiguous()
-
-    def _encoder(self, wv: _Wave, plan: TilePlan, img: torch.Tensor, res: torch.Tensor):
-        cfg, ws, W, st = self.cfg, self.ws, self.w, wv.st
-        ch, mult, nres = cfg["ch"], tuple(cfg["ch_mult"]), cfg["num_res_blocks"]
-        nb, h, w, p, c = wv.nb, wv.h, wv.w, "encoder.", cfg["ch"]
-        x_in = self._gather(wv, plan, img)
-        st["cur"] = self._new(nb * h * w, c)
-        lib.conv3x3_small_cin(x_in, None, x_in.shape[1], 0, nb, h, w, W[p + "conv_in.weight"], W[p + "conv_in.bias"],
-                              c, st["cur"])
-        del x_in
-        self._emit(wv, st["cur"], c, h, w)
-        for lvl in range(len(mult)):
-            cout = ch * mult[lvl]
-            down = lvl != len(mult) - 1
-            for j in range(nres):
-                yield from self._res(wv, f"{p}down.{lvl}.block.{j}.", c, cout, h, w, emit=not (down and j == nres - 1))
-                c = cout
-            if down:
-                ho, wo = h // 2, w // 2
-                col = ws.get("a16", (nb * ho * wo, 9 * c), self.op_dtype)
-                lib.im2col_s2(st["cur"], nb, h, w, c, 0, col)
-                st["cur"] = self._new(nb * ho * wo, c)
-                lib.gemm(col, W[f"{p}down.{lvl}.downsample.conv.weight"], st["cur"], M=nb * ho * wo, N=c, K=9 * c,
-                         bias=W[f"{p}down.{lvl}.downsample.conv.bias"], split_k=1)
-                h, w = ho, wo
-                self._emit(wv, st["cur"], c, h, w)
-        yield from self._mid(wv, p, c, h, w)
-        stats = yield h * w
-        a16 = ws.get("a16", (nb * h * w, c), self.op_dtype)
-        lib.gn_apply(st.pop("cur"), None, c, 0, nb, h, w, stats, W[p + "norm_out.weight"], W[p + "norm_out.bias"],
-                     a16, norm=True, silu=True)
-        zc2 = 2 * cfg["z_channels"]
-        m = self._new(nb, h, w, zc2)
-        lib.conv3x3_small_cout(a16, nb, h, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], zc2, m, nchw=False)
+    def _tiles(self, wv: _Wave, plan: TilePlan, src: torch.Tensor, res: torch.Tensor, decoder: bool):
+        """The wave's tiles through VaeWalk: gathered as one NCHW batch, tile-major (entry = tile * N + image), and
+        each tile's output cropped to its box of `res` (NCHW for the decoder, NHWC for the encoder)."""
+        walk = VaeWalk(self.base, wv.st, self._new, self.ws, wv.nb)
+        boxes = [plan.in_boxes[t] for t in wv.tiles]
+        out = yield from (walk.decoder if decoder else walk.encoder)(
+            torch.cat([src[:, :, y0:y1, x0:x1] for x0, x1, y0, y1 in boxes], 0).contiguous())
         n_img = res.shape[0]
         for i, t in enumerate(wv.tiles):
             x0, x1, y0, y1 = plan.out_boxes[t]
             cy, cx = plan.crops[t]
-            res[:, y0:y1, x0:x1] = m[i * n_img:(i + 1) * n_img, cy:cy + y1 - y0, cx:cx + x1 - x0]
-
-    def _decoder(self, wv: _Wave, plan: TilePlan, z: torch.Tensor, res: torch.Tensor):
-        cfg, ws, W, st = self.cfg, self.ws, self.w, wv.st
-        ch, mult, nres = cfg["ch"], tuple(cfg["ch_mult"]), cfg["num_res_blocks"]
-        nb, h, w, p = wv.nb, wv.h, wv.w, "decoder."
-        c = ch * mult[-1]
-        z_in = self._gather(wv, plan, z)
-        st["cur"] = self._new(nb * h * w, c)
-        lib.conv3x3_small_cin(z_in, None, z_in.shape[1], 0, nb, h, w, W[p + "conv_in.weight"], W[p + "conv_in.bias"],
-                              c, st["cur"])
-        del z_in
-        self._emit(wv, st["cur"], c, h, w)
-        yield from self._mid(wv, p, c, h, w)
-        for lvl in reversed(range(len(mult))):
-            cout = ch * mult[lvl]
-            for j in range(nres + 1):
-                yield from self._res(wv, f"{p}up.{lvl}.block.{j}.", c, cout, h, w, emit=not (lvl != 0 and j == nres))
-                c = cout
-            if lvl != 0:
-                up16 = ws.get("a16", (nb * 4 * h * w, c), self.op_dtype)
-                lib.gn_apply(st["cur"], None, c, 0, nb, h, w, None, None, None, up16, norm=False, silu=False, upsample=2)
-                h, w = 2 * h, 2 * w
-                st["cur"] = self._new(nb * h * w, c)
-                self._conv(wv, up16, f"{p}up.{lvl}.upsample.conv", st["cur"], c, c, h, w)
-        stats = yield h * w
-        a16 = ws.get("a16", (nb * h * w, c), self.op_dtype)
-        lib.gn_apply(st.pop("cur"), None, c, 0, nb, h, w, stats, W[p + "norm_out.weight"], W[p + "norm_out.bias"],
-                     a16, norm=True, silu=True)
-        out = self._new(nb, cfg["out_ch"], h, w)
-        lib.conv3x3_small_cout(a16, nb, h, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], cfg["out_ch"], out,
-                               nchw=True)
-        n_img = res.shape[0]
-        for i, t in enumerate(wv.tiles):
-            x0, x1, y0, y1 = plan.out_boxes[t]
-            cy, cx = plan.crops[t]
-            res[:, :, y0:y1, x0:x1] = out[i * n_img:(i + 1) * n_img, :, cy:cy + y1 - y0, cx:cx + x1 - x0]
+            tile = out[i * n_img:(i + 1) * n_img]
+            if decoder:
+                res[:, :, y0:y1, x0:x1] = tile[:, :, cy:cy + y1 - y0, cx:cx + x1 - x0]
+            else:
+                res[:, y0:y1, x0:x1] = tile[:, cy:cy + y1 - y0, cx:cx + x1 - x0]
