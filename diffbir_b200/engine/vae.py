@@ -185,6 +185,13 @@ class VaeWalk:
         self.w, self.cfg, self.dev, self.op_dtype = eng.w, eng.cfg, eng.dev, eng.op_dtype
         self.st, self.new, self.ws, self.nb = st, new, ws, nb
 
+    @staticmethod
+    def stops(cfg: dict, decoder: bool) -> int:
+        """GroupNorms the encoder / decoder stops at, known without running a walk: two per ResnetBlock (the levels'
+        blocks, and the mid block's two), one for the mid attention, one before conv_out. 22 / 30 for the SD VAE."""
+        blocks = len(cfg["ch_mult"]) * (cfg["num_res_blocks"] + (1 if decoder else 0)) + 2
+        return 2 * blocks + 2
+
     def _conv(self, a16, key, out, cin, cout, h, w, residual=None, partials=True):
         """3x3 implicit-GEMM convolution into `out`. Returns the (partials, slots) to yield at the GroupNorm of
         `out`: NO_PARTIALS when they are not asked for (`out` feeds a resampling, not a GroupNorm) or the GEMM

@@ -19,6 +19,11 @@ that at each stop takes every wave's moments, merges them and sends the statisti
 carries its state (the current fp32 tensor and the pending residual, fresh `torch.empty` tensors in the wave's
 `st`); beyond `state_budget` bytes the state is staged through pinned host buffers on a side stream, overlapped
 with the next wave. Launches are eager (no CUDA graphs).
+
+Cooperating ranks (`TiledVae(base, rank, world)`, all called with the same input) split the tiles
+(`tiles_of_ranks`): each runs its own as above; at every GroupNorm the ranks all-gather their entries' fp64 moments
+and pixel counts into the global moment buffer and run the same merge, and after the last one they all-gather the
+output boxes. A tile's bits do not depend on its wave, so every rank returns the single-rank result bit for bit.
 """
 from __future__ import annotations
 
@@ -27,6 +32,7 @@ from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Tuple
 
 import torch
+import torch.distributed as dist
 
 from .. import lib
 from .common import Workspace
@@ -102,6 +108,103 @@ def whole_image_plan(h: int, w: int, is_decoder: bool) -> TilePlan:
     return TilePlan([(0, w, 0, h)], [(0, ow, 0, oh)], [(0, 0)], {(h, w): [0]})
 
 
+# ---- tiles sharded over cooperating ranks (host logic, shared with the CPU / gloo tests) ----
+def tiles_of_ranks(plan: TilePlan, world: int) -> List[List[int]]:
+    """Each rank's tiles, ascending. Greedy by full-resolution pixels (a tile's input box scaled by a constant):
+    the largest tile first, ties by tile index, each to the rank with the fewest pixels so far, ties to the lowest
+    rank. A pure function of the plan, so every rank computes the same split, and the most loaded rank exceeds the
+    least loaded by at most one tile. World 1 owns every tile in plan order; ranks beyond the tile count own none."""
+    area = [(x1 - x0) * (y1 - y0) for x0, x1, y0, y1 in plan.in_boxes]
+    load, owned = [0] * world, [[] for _ in range(world)]
+    for t in sorted(range(len(area)), key=lambda t: (-area[t], t)):
+        r = min(range(world), key=lambda r: (load[r], r))
+        load[r] += area[t]
+        owned[r].append(t)
+    return [sorted(o) for o in owned]
+
+
+def entries_of_ranks(owned: List[List[int]], n_img: int) -> List[List[int]]:
+    """The batch entries (entry = tile * n_img + image) of each rank's tiles, in its tile order."""
+    return [[t * n_img + b for t in tiles for b in range(n_img)] for tiles in owned]
+
+
+def moment_rows(entries: List[List[int]], slots: int) -> List[int]:
+    """Row of every global entry in the gathered moment payloads viewed as [world * slots, ...]."""
+    rows = [0] * sum(map(len, entries))
+    for r, ents in enumerate(entries):
+        for s, e in enumerate(ents):
+            rows[e] = r * slots + s
+    return rows
+
+
+MOMENT_COLS = 65        # one payload row: 32 groups x (mean, biased variance), then the entry's pixel count; fp64
+
+
+def pack_moments(moments: torch.Tensor, mine: torch.Tensor, pixels: torch.Tensor, slots: int) -> torch.Tensor:
+    """A rank's payload at one GroupNorm: row s holds its entry mine[s] (global index) -- the fp64 moments of
+    `moments` [entries, 32, 2] and the pixel count pixels[s] -- and rows past its entries are zero."""
+    k = mine.numel()
+    send = moments.new_zeros(slots, MOMENT_COLS)
+    send[:k, :64] = moments.index_select(0, mine).view(k, 64)
+    send[:k, 64] = pixels
+    return send
+
+
+def unpack_moments(recv: torch.Tensor, rows: torch.Tensor, moments: torch.Tensor) -> torch.Tensor:
+    """Every rank's payload, recv [world, slots, MOMENT_COLS], into the global moments [entries, 32, 2]: every entry
+    is rewritten from its owner's row (`moment_rows`). Returns the entries' pixel counts, int64."""
+    flat = recv.view(-1, MOMENT_COLS).index_select(0, rows)
+    moments.copy_(flat[:, :64].view(moments.shape))
+    return flat[:, 64].long()
+
+
+def _box(res: torch.Tensor, box: Tuple[int, int, int, int], nchw: bool) -> torch.Tensor:
+    x0, x1, y0, y1 = box
+    return res[:, :, y0:y1, x0:x1] if nchw else res[:, y0:y1, x0:x1]
+
+
+def box_share(res: torch.Tensor, boxes: List[Tuple[int, int, int, int]], nchw: bool) -> int:
+    """Elements of `res` (all images, all channels) inside the output boxes."""
+    return sum(_box(res, b, nchw).numel() for b in boxes)
+
+
+def pack_boxes(res: torch.Tensor, boxes: List[Tuple[int, int, int, int]], size: int, nchw: bool) -> torch.Tensor:
+    """The output boxes of a rank's tiles, copied from `res` (NCHW or NHWC) one after the other into a flat buffer of
+    `size` elements (the largest rank's share); the padding is not written and never read."""
+    send = res.new_empty(size)
+    off = 0
+    for b in boxes:
+        v = _box(res, b, nchw)
+        send[off:off + v.numel()].view(v.shape).copy_(v)
+        off += v.numel()
+    return send
+
+
+def unpack_boxes(recv: torch.Tensor, res: torch.Tensor, boxes: List[List[Tuple[int, int, int, int]]], nchw: bool,
+                 skip: int = -1) -> None:
+    """Copies every rank's boxes from the gathered buffers recv [world, size] into `res`, except rank `skip`'s."""
+    for r, rb in enumerate(boxes):
+        if r == skip:
+            continue
+        off = 0
+        for b in rb:
+            v = _box(res, b, nchw)
+            v.copy_(recv[r, off:off + v.numel()].view(v.shape))
+            off += v.numel()
+
+
+class ProcessGroupGather:
+    """The collective of the sharded tiled VAE: all-gather of equal-size tensors over the torch.distributed default
+    group (NCCL between GPUs). t [...] on every rank -> [world, ...], rank r's tensor at r. Gathered flat, the form
+    every backend takes."""
+
+    def all_gather(self, t: torch.Tensor) -> torch.Tensor:
+        world = dist.get_world_size()
+        out = torch.empty(world * t.numel(), dtype=t.dtype, device=t.device)
+        dist.all_gather_into_tensor(out, t.contiguous().view(-1))
+        return out.view((world,) + tuple(t.shape))
+
+
 class _Wave:
     """Tiles of one shape class that run together; entry j = (tile j // N, image j % N)."""
 
@@ -126,8 +229,14 @@ class TiledVae:
     # working buffers to a few GiB at the full config (128 channels at full resolution).
     wave_pixels: int = 1 << 22
 
-    def __init__(self, base: VaeEngine):
+    def __init__(self, base: VaeEngine, rank: int = 0, world: int = 1, comm=None):
+        """world > 1: this is rank `rank` of cooperating ranks that all call with the same input. Each runs its own
+        tiles (`tiles_of_ranks`); `comm.all_gather` (default: `ProcessGroupGather`) exchanges the tiles' GroupNorm
+        moments at every stop and their outputs at the end, so every rank returns the full result, with the bits
+        of one rank. Inputs that run un-tiled stay replicated."""
         self.base, self.cfg, self.dev = base, base.cfg, base.dev
+        self.rank, self.world = rank, world
+        self.comm = comm if comm is not None or world == 1 else ProcessGroupGather()
         self.ws = Workspace(self.dev)
         self.last_stats: dict = {}
 
@@ -137,7 +246,8 @@ class TiledVae:
         """img fp32 NCHW [N, 3, H, W] in [-1, 1], tile_size in image pixels -> moments fp32 [N, 8, H/8, W/8]."""
         assert img.is_cuda and img.dtype == torch.float32 and img.is_contiguous()
         n, _, h, w = img.shape
-        if max(h, w) <= 2 * PAD_ENCODER + tile_size:
+        tiled = max(h, w) > 2 * PAD_ENCODER + tile_size
+        if not tiled:
             if (h // 8) * (w // 8) % 8 == 0:
                 return self.base.encode_moments(img)
             plan = whole_image_plan(h, w, False)      # a latent the un-tiled engine's attention cannot take
@@ -145,7 +255,7 @@ class TiledVae:
             plan = plan_vae_tiles(h, w, tile_size, False)
         zc2 = 2 * self.cfg["z_channels"]
         res = torch.empty(n, h // 8, w // 8, zc2, dtype=torch.float32, device=self.dev)      # NHWC
-        self._run(plan, img, res, False)
+        self._run(plan, img, res, False, tiled and self.world > 1)
         return self.base.quant(res, self._new)
 
     @torch.no_grad()
@@ -154,7 +264,8 @@ class TiledVae:
         image fp32 NCHW [N, 3, 8h, 8w]."""
         assert z.is_cuda and z.dtype == torch.float32 and z.is_contiguous()
         n, zc, h, w = z.shape
-        if max(h, w) <= 2 * PAD_DECODER + tile_size:
+        tiled = max(h, w) > 2 * PAD_DECODER + tile_size
+        if not tiled:
             if h * w % 8 == 0:
                 return self.base.decode(z)
             plan = whole_image_plan(h, w, True)
@@ -162,26 +273,38 @@ class TiledVae:
             plan = plan_vae_tiles(h, w, tile_size, True)
         z2n = self.base.post_quant(z, self._new)
         res = torch.empty(n, self.cfg["out_ch"], 8 * h, 8 * w, dtype=torch.float32, device=self.dev)
-        self._run(plan, z2n, res, True)
+        self._run(plan, z2n, res, True, tiled and self.world > 1)
         return res
 
     def release_buffers(self) -> None:
         self.ws.clear()
 
     # ------------------------------------------------------------------ waves, merge and state staging
-    def _waves(self, plan: TilePlan, n_img: int, up: int) -> List[_Wave]:
-        waves = []
+    def _waves(self, plan: TilePlan, n_img: int, up: int, mine: List[int]) -> List[_Wave]:
+        waves, mine = [], set(mine)
         for shape, tiles in plan.classes.items():
+            tiles = [t for t in tiles if t in mine]
             full = n_img * shape[0] * shape[1] * up * up
             per = max(1, self.wave_pixels // full)
             for i in range(0, len(tiles), per):
                 waves.append(_Wave(tiles[i:i + per], n_img, shape, self.dev))
         return waves
 
-    def _run(self, plan: TilePlan, src: torch.Tensor, res: torch.Tensor, decoder: bool) -> None:
+    def _run(self, plan: TilePlan, src: torch.Tensor, res: torch.Tensor, decoder: bool, shard: bool) -> None:
+        """Runs the plan's tiles into `res`. shard: this rank runs its own tiles only; at every stop the ranks
+        all-gather their entries' moments and pixel counts into the global moment buffer before the same merge,
+        and after the last one their output boxes. Every rank issues the same collectives, tiles or not."""
         n_img = src.shape[0]
-        waves = self._waves(plan, n_img, 8 if decoder else 1)
+        owned = tiles_of_ranks(plan, self.world if shard else 1)
+        rank = self.rank if shard else 0
+        waves = self._waves(plan, n_img, 8 if decoder else 1, owned[rank])
         entries = len(plan.in_boxes) * n_img
+        stops = VaeWalk.stops(self.cfg, decoder)
+        if shard:
+            ents = entries_of_ranks(owned, n_img)
+            share = max(map(len, ents))                  # payload rows per rank
+            mine = torch.tensor(ents[rank], dtype=torch.int64).to(self.dev)
+            rows = torch.tensor(moment_rows(ents, share), dtype=torch.int64).to(self.dev)
         self._moments = torch.empty(entries, 32, 2, dtype=torch.float64, device=self.dev)
         stats = torch.empty(entries, 64, dtype=torch.float32, device=self.dev)
         image = (torch.arange(entries, dtype=torch.int32) % n_img).to(self.dev)
@@ -215,21 +338,34 @@ class TiledVae:
                     else:
                         self._spill(wv, main)
                         spills += 1
-                if done:
-                    assert done == len(waves), "waves of one network must reach the same GroupNorms"
+                if passes == stops:
+                    assert done == len(waves), "the walk has more GroupNorms than VaeWalk.stops"
                     break
+                assert not done, "the walk has fewer GroupNorms than VaeWalk.stops"
                 key = tuple(pix)
                 if key not in pix_cache:
-                    per_entry = [p for wv, p in zip(waves, pix) for _ in range(wv.nb)]
-                    order = torch.cat([wv.entries.cpu() for wv in waves]).long()
                     arr = torch.empty(entries, dtype=torch.int64)
-                    arr[order] = torch.tensor(per_entry, dtype=torch.int64)
-                    pix_cache[key] = arr.to(self.dev)
+                    for wv, p in zip(waves, pix):
+                        arr[wv.entries.cpu().long()] = p
+                    # sharded: the pixel counts of this rank's entries, in its payload's row order
+                    pix_cache[key] = (arr[ents[rank]].double() if shard else arr).to(self.dev)
+                pixels = pix_cache[key]
+                if shard:
+                    # a rank sees only its own shape classes: the counts travel with the moments, so every rank
+                    # merges the same global buffer with the same weights
+                    pixels = unpack_moments(self.comm.all_gather(pack_moments(self._moments, mine, pixels, share)),
+                                            rows, self._moments)
                 # the reference visits the tiles forwards at even GroupNorms and backwards at odd ones
-                lib.gn_merge(self._moments, pix_cache[key], image, entries, n_img, stats, reverse=passes % 2 == 1)
+                lib.gn_merge(self._moments, pixels, image, entries, n_img, stats, reverse=passes % 2 == 1)
                 for i, wv in enumerate(waves):
                     sent[i] = stats.index_select(0, wv.entries.long())
                 passes += 1
+            if shard:
+                # the output boxes partition `res`: copies, so every element keeps its owner's bits
+                boxes = [[plan.out_boxes[t] for t in tiles] for tiles in owned]
+                size = max(box_share(res, b, decoder) for b in boxes)
+                recv = self.comm.all_gather(pack_boxes(res, boxes[rank], size, decoder))
+                unpack_boxes(recv, res, boxes, decoder, skip=rank)
         finally:
             torch.cuda.current_stream(self.dev).wait_stream(self._side)
             self._side.synchronize()
@@ -241,8 +377,8 @@ class TiledVae:
             self._moments = None
             if spills:
                 torch._C._host_emptyCache()       # the pinned staging buffers live for one call
-        self.last_stats = dict(tiles=len(plan.in_boxes), waves=len(waves), groupnorms=passes, spills=spills,
-                               budget=budget)
+        self.last_stats = dict(tiles=len(plan.in_boxes), owned=len(owned[rank]), waves=len(waves), groupnorms=passes,
+                               exchanges=passes + 1 if shard else 0, spills=spills, budget=budget)
 
     def _spill(self, wv: _Wave, main) -> None:
         """Copies the wave's state to its pinned host buffer on the side stream and drops the device copy."""

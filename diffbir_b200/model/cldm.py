@@ -45,8 +45,9 @@ class ControlLDM:
         self._ctx_ref = None      # (tensor, version) the engine's cross-attention K/V were built from
         self._t_key = None
         self._txt_cache: Dict[str, torch.Tensor] = {}   # prompt -> [77, D] text-tower output (see encode_text)
-        # True: VAE encode / decode are sharded by image rows over the torch.distributed ranks (all ranks must pass
-        # the same tensors; set by the pipeline while ranks cooperate on one job: tiled / batch-sharded sampling)
+        # True: VAE encode / decode are sharded over the torch.distributed ranks, by image rows un-tiled and by tiles
+        # tiled (all ranks must pass the same tensors; set by the pipeline while ranks cooperate on one job: tiled /
+        # batch-sharded sampling)
         self.shard_vae = False
         self._svae = None
         self._tvae = None
@@ -194,12 +195,15 @@ class ControlLDM:
         return sv.decode(z) if sv is not None else self.vae.decode(z)
 
     def tiled_vae(self):
-        """The tiled VAE (engine.vae_tiled) on this model's VAE weights. It runs on each rank by itself: the
-        row-sharded VAE computes the un-tiled semantics."""
+        """The tiled VAE (engine.vae_tiled) on this model's VAE weights. While shard_vae is set and more than one
+        rank cooperates, each rank runs its share of the tiles and every rank returns the full result (the
+        row-sharded VAE computes the un-tiled semantics, so it is not used here); otherwise it runs by itself."""
         self._build()
-        if self._tvae is None:
+        import torch.distributed as dist
+        world = dist.get_world_size() if self.shard_vae and dist.is_available() and dist.is_initialized() else 1
+        if self._tvae is None or self._tvae.world != world:
             from ..engine.vae_tiled import TiledVae
-            self._tvae = TiledVae(self.vae)
+            self._tvae = TiledVae(self.vae, dist.get_rank() if world > 1 else 0, world)
         return self._tvae
 
     def _sharded_vae(self, h_img: int, w_img: int):

@@ -63,7 +63,7 @@ class Pipeline:
         self.output_size: Tuple[int, int] = None
         self.taps: Optional[dict] = None   # set to {} to capture intermediates (tests)
         self.fused_post = True             # colour fix + quantisation as one kernel (False: the torch op sequence)
-        self.shard_vae = True              # cooperating ranks (tiled / batch-sharded sampling) shard the VAE by image rows
+        self.shard_vae = True              # cooperating ranks (tiled / batch-sharded sampling) shard the VAE (by image rows or by tiles)
         self.shard_batch = False           # un-tiled batches: shard (image, CFG branch) forwards over torch.distributed ranks
         self.max_tile_forwards = 128       # tiled sampling: most tile-forwards x images per graph replay (Sampler.max_tile_forwards)
         self.marks: Optional[list] = None  # set to [] to record (phase, CUDA event) boundaries (bench.py phases_ms)
@@ -100,8 +100,8 @@ class Pipeline:
         cond_img = pad_to_multiples_of(cond_img, multiple=64 if not vae_encoder_tiled and not cldm_tiled else 8)
         vae_encoder_tiled, vae_decoder_tiled = vae_tiling(cond_img.shape[2:], vae_encoder_tiled, vae_encoder_tile_size,
                                                           vae_decoder_tiled, vae_decoder_tile_size)
-        # ranks that cooperate on this job (sharded tiles or batch units) also shard the un-tiled VAE by image rows;
-        # a tiled VAE runs replicated on every rank (ControlLDM)
+        # ranks that cooperate on this job (sharded tiles or batch units) also shard the VAE: the un-tiled one by
+        # image rows, the tiled one by tiles (ControlLDM)
         import torch.distributed as dist
         coop = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and (cldm_tiled or self.shard_batch)
         self.cldm.shard_vae = bool(coop and self.shard_vae)
