@@ -424,3 +424,110 @@ def scunet_shapes(cfg: dict) -> Shapes:
             s[f"{name}.{nblk}.weight"] = (2 * c, c, 2, 2)
     s["m_tail.0.weight"] = (cfg["in_nc"], d, 3, 3)
     return s
+
+
+# ------------------------------------------------------------------------------- RAM++ (captioner)
+# RAM_plus(image_size=384, vit="swin_l") (ram/models/ram_plus.py:90-179): Swin-L at 384^2 (configs/swin/
+# config_swinL_384.json), the 2-layer cross-attention-only BERT tagging head (configs/q2l_config.json,
+# encoder_width 512) and 4585 classes x 51 description embeddings.
+RAM_CFG = dict(img_size=384, patch_size=4, embed_dim=192, depths=(2, 2, 18, 2), num_heads=(6, 12, 24, 48),
+               window_size=12, mlp_ratio=4, vision_width=1536, embed=512, hidden=768, bert_heads=4,
+               intermediate=3072, bert_layers=2, num_class=4585, des_per_class=51)
+
+
+def ram_stages(cfg: dict):
+    """(channels, token-map side, heads, window, block shifts) per Swin stage. A stage whose map is no larger than
+    the window runs one un-shifted window of the map's size (swin_transformer.py:195-198)."""
+    out = []
+    side = cfg["img_size"] // cfg["patch_size"]
+    for i, (depth, heads) in enumerate(zip(cfg["depths"], cfg["num_heads"])):
+        r = side >> i
+        ws, shift = cfg["window_size"], cfg["window_size"] // 2
+        if r <= ws:
+            ws, shift = r, 0
+        out.append((cfg["embed_dim"] << i, r, heads, ws, tuple(0 if b % 2 == 0 else shift for b in range(depth))))
+    return out
+
+
+def ram_shapes(cfg: dict) -> Shapes:
+    """Parameters of RAM_plus in its state_dict order, without the relative_position_index / attn_mask buffers
+    the checkpoint loader drops (ram/models/utils.py:241-270)."""
+    s: Shapes = OrderedDict()
+    e, hid, inter = cfg["embed"], cfg["hidden"], cfg["intermediate"]
+    s["label_embed"] = (cfg["num_class"] * cfg["des_per_class"], e)
+    s["reweight_scale"] = ()
+    c0, p = cfg["embed_dim"], "visual_encoder."
+    s[p + "patch_embed.proj.weight"] = (c0, 3, cfg["patch_size"], cfg["patch_size"])
+    s[p + "patch_embed.proj.bias"] = (c0,)
+    s[p + "patch_embed.norm.weight"] = (c0,)
+    s[p + "patch_embed.norm.bias"] = (c0,)
+    stages = ram_stages(cfg)
+    for i, (c, _, heads, ws, shifts) in enumerate(stages):
+        for b in range(len(shifts)):
+            q = f"{p}layers.{i}.blocks.{b}."
+            s[q + "norm1.weight"] = (c,)
+            s[q + "norm1.bias"] = (c,)
+            s[q + "attn.relative_position_bias_table"] = ((2 * ws - 1) ** 2, heads)
+            s[q + "attn.qkv.weight"] = (3 * c, c)
+            s[q + "attn.qkv.bias"] = (3 * c,)
+            s[q + "attn.proj.weight"] = (c, c)
+            s[q + "attn.proj.bias"] = (c,)
+            s[q + "norm2.weight"] = (c,)
+            s[q + "norm2.bias"] = (c,)
+            s[q + "mlp.fc1.weight"] = (cfg["mlp_ratio"] * c, c)
+            s[q + "mlp.fc1.bias"] = (cfg["mlp_ratio"] * c,)
+            s[q + "mlp.fc2.weight"] = (c, cfg["mlp_ratio"] * c)
+            s[q + "mlp.fc2.bias"] = (c,)
+        if i < len(stages) - 1:
+            s[f"{p}layers.{i}.downsample.reduction.weight"] = (2 * c, 4 * c)
+            s[f"{p}layers.{i}.downsample.norm.weight"] = (4 * c,)
+            s[f"{p}layers.{i}.downsample.norm.bias"] = (4 * c,)
+    s[p + "norm.weight"] = (cfg["vision_width"],)
+    s[p + "norm.bias"] = (cfg["vision_width"],)
+    for l in range(cfg["bert_layers"]):
+        q = f"tagging_head.encoder.layer.{l}."
+        s[q + "crossattention.self.query.weight"] = (hid, hid)
+        s[q + "crossattention.self.query.bias"] = (hid,)
+        s[q + "crossattention.self.key.weight"] = (hid, e)
+        s[q + "crossattention.self.key.bias"] = (hid,)
+        s[q + "crossattention.self.value.weight"] = (hid, e)
+        s[q + "crossattention.self.value.bias"] = (hid,)
+        s[q + "crossattention.output.dense.weight"] = (hid, hid)
+        s[q + "crossattention.output.dense.bias"] = (hid,)
+        s[q + "crossattention.output.LayerNorm.weight"] = (hid,)
+        s[q + "crossattention.output.LayerNorm.bias"] = (hid,)
+        s[q + "intermediate.dense.weight"] = (inter, hid)
+        s[q + "intermediate.dense.bias"] = (inter,)
+        s[q + "output.dense.weight"] = (hid, inter)
+        s[q + "output.dense.bias"] = (hid,)
+        s[q + "output.LayerNorm.weight"] = (hid,)
+        s[q + "output.LayerNorm.bias"] = (hid,)
+    s["wordvec_proj.weight"] = (hid, e)
+    s["wordvec_proj.bias"] = (hid,)
+    s["fc.weight"] = (1, hid)
+    s["fc.bias"] = (1,)
+    s["image_proj.weight"] = (e, cfg["vision_width"])
+    s["image_proj.bias"] = (e,)
+    return s
+
+
+def ram_state_dict(ckpt: dict, cfg: dict = None) -> dict:
+    """The strict RAM++ loader: unwraps the checkpoint's `model` entry, drops the relative_position_index / attn_mask
+    buffers and renames vision_multi -> tagging_head as ram/models/utils.py:241-270 does, then checks every key and
+    shape of ram_shapes. A relative-position bias table of another window size is refused (the reference would
+    interpolate it; the Swin-L checkpoint already holds 23^2-row tables)."""
+    cfg = RAM_CFG if cfg is None else cfg
+    sd = ckpt["model"] if "model" in ckpt else ckpt
+    sd = {k.replace("vision_multi", "tagging_head"): v for k, v in sd.items()
+          if "relative_position_index" not in k and "attn_mask" not in k}
+    rows = (2 * cfg["window_size"] - 1) ** 2
+    for k, v in sd.items():
+        if k.endswith("relative_position_bias_table") and v.shape[0] != rows:
+            raise ValueError(f"{k}: {v.shape[0]} rows, expected {rows} ((2 * {cfg['window_size']} - 1)^2); "
+                             "relative-position tables of other window sizes are not interpolated")
+    for k, shp in ram_shapes(cfg).items():
+        if k not in sd:
+            raise KeyError(f"RAM++ checkpoint is missing {k}")
+        if tuple(sd[k].shape) != tuple(shp):
+            raise ValueError(f"{k}: {tuple(sd[k].shape)} != {shp}")
+    return sd

@@ -399,9 +399,10 @@ gn_apply_kernel(const float* __restrict__ s1, const float* __restrict__ s2, int 
   }
 }
 
-// LayerNorm over the last dim; one warp per row; C <= 1280, C % 4 == 0.
-// Output op16 with row stride ldo >= C; columns [C, ldo) are zero-filled (K padding).
-template <bool F32OUT>
+// LayerNorm over the last dim; one warp per row; C <= 32 * 4 * MAXV, C % 4 == 0 (MAXV 10: C <= 1280; MAXV 12:
+// the 1536-wide stage 4 of Swin-L in RAM++). Output op16 with row stride ldo >= C; columns [C, ldo) are zero-filled
+// (K padding).
+template <bool F32OUT, int MAXV>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const float* __restrict__ x, long long ldx, int rows, int C,
                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
@@ -416,7 +417,6 @@ layernorm_kernel(const float* __restrict__ x, long long ldx, int rows, int C,
     gamma += goff; beta += goff;
   }
   const float* xr = x + row * ldx;
-  constexpr int MAXV = 10;
   float4 v[MAXV];
   float s = 0.f;
 #pragma unroll
@@ -579,16 +579,26 @@ extern "C" int dbir_layernorm(const float* x, int64_t ldx, int32_t rows, int32_t
                               const float* gamma, const float* beta, float eps, void* out,
                               int64_t ldo, int32_t out_kind, int32_t rows_per_group, void* stream) {
   DBIR_REQUIRE(x && gamma && beta && out, "dbir_layernorm: null pointer");
-  DBIR_REQUIRE(c % 4 == 0 && c <= 1280 && ldo >= c && ldo % 4 == 0 && ldo <= 1280,
+  DBIR_REQUIRE(c % 4 == 0 && c <= 1536 && ldo >= c && ldo % 4 == 0 && ldo <= (c <= 1280 ? 1280 : 1536),
                "dbir_layernorm: unsupported width %d (ldo %lld)", c, (long long)ldo);
   const int rows_per_cta = 8;
   const int grid = (rows + rows_per_cta - 1) / rows_per_cta;
   const long long ldx_ = ldx, ldo_ = ldo;
-  if (out_kind == 0)
-    DBIR_CHECK_CUDA(dbir_launch(layernorm_kernel<true>, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                                x, ldx_, rows, c, gamma, beta, eps, out, ldo_, rows_per_group));
-  else
-    DBIR_CHECK_CUDA(dbir_launch(layernorm_kernel<false>, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                                x, ldx_, rows, c, gamma, beta, eps, out, ldo_, rows_per_group));
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (c <= 1280) {
+    if (out_kind == 0)
+      DBIR_CHECK_CUDA(dbir_launch(layernorm_kernel<true, 10>, dim3(grid), dim3(256), 0, st,
+                                  x, ldx_, rows, c, gamma, beta, eps, out, ldo_, rows_per_group));
+    else
+      DBIR_CHECK_CUDA(dbir_launch(layernorm_kernel<false, 10>, dim3(grid), dim3(256), 0, st,
+                                  x, ldx_, rows, c, gamma, beta, eps, out, ldo_, rows_per_group));
+  } else {
+    if (out_kind == 0)
+      DBIR_CHECK_CUDA(dbir_launch(layernorm_kernel<true, 12>, dim3(grid), dim3(256), 0, st,
+                                  x, ldx_, rows, c, gamma, beta, eps, out, ldo_, rows_per_group));
+    else
+      DBIR_CHECK_CUDA(dbir_launch(layernorm_kernel<false, 12>, dim3(grid), dim3(256), 0, st,
+                                  x, ldx_, rows, c, gamma, beta, eps, out, ldo_, rows_per_group));
+  }
   return 0;
 }

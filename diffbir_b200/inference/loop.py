@@ -16,6 +16,7 @@ import torch
 import yaml
 from PIL import Image
 
+from ..utils.caption import Captioner, EmptyCaptioner
 from ..utils.common import instantiate_from_config
 from .pretrained_models import default_weights_dir, resolve
 
@@ -85,7 +86,7 @@ def check_supported(args: Namespace) -> None:
         raise NotImplementedError(f"--device {args.device}: the engines are CUDA (sm_90a) only, there is no CPU path")
     if args.sampler not in SUPPORTED_SAMPLERS:
         raise NotImplementedError(f"--sampler {args.sampler}: not one of {SUPPORTED_SAMPLERS}")
-    if args.captioner != "none":
+    if args.captioner not in ("none", "ram"):
         raise NotImplementedError(f"--captioner {args.captioner}: captioners are outside the path; pass --captioner none "
                                   "and a --pos_prompt")
     if args.guidance:
@@ -98,7 +99,14 @@ def check_supported(args: Namespace) -> None:
         raise NotImplementedError("Tiled-VAE is outside the path (SURVEY.md §8f); the VAE engines run un-tiled")
 
 
+def prompt_with_caption(caption: str, pos_prompt: str) -> str:
+    """loop.py:167-169: the caption, then the user's positive prompt, empty parts dropped."""
+    return ", ".join([text for text in [caption, pos_prompt] if text])
+
+
 class InferenceLoop:
+    captioner: Captioner = EmptyCaptioner("cuda")      # replaced by load_captioner
+
     def __init__(self, args: Namespace) -> None:
         self.args = args
         check_supported(args)
@@ -108,6 +116,7 @@ class InferenceLoop:
         self.synthetic = bool(getattr(args, "synthetic", False))
         self.load_cleaner()
         self.load_cldm()
+        self.load_captioner()
         self.cond_fn = None
         self.load_pipeline()
 
@@ -117,6 +126,14 @@ class InferenceLoop:
 
     def load_pipeline(self) -> None:
         raise NotImplementedError
+
+    def load_captioner(self) -> None:
+        """loop.py:119-129: --captioner none -> no caption, ram -> RAM++ tags on the engine."""
+        if self.args.captioner == "ram":
+            from ..utils.caption import RAMCaptioner
+            self.captioner = RAMCaptioner(self.args.device, self.weights_dir, self.synthetic, self.args.seed)
+        else:
+            self.captioner = EmptyCaptioner(self.args.device)
 
     def _operand_check(self) -> None:
         from .. import lib
@@ -187,7 +204,8 @@ class InferenceLoop:
         a = self.args
         self.setup()
         for lq in self.load_lq():
-            pos_prompt = ", ".join([text for text in ["", a.pos_prompt] if text])     # caption is empty (captioner none)
+            caption = self.captioner(lq)                 # fp32 logits; nothing here runs under autocast
+            pos_prompt = prompt_with_caption(caption, a.pos_prompt)
             neg_prompt = a.neg_prompt
             lq = self.after_load_lq(lq)
             n_samples, batch_size = a.n_samples, a.batch_size

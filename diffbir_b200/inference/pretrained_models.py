@@ -22,6 +22,8 @@ MODELS: Dict[str, str] = {
     "v1_general": "v1_general.pth",
     "v2": "v2.pth",
     "v2.1": "DiffBIR_v2.1.pt",
+    # captioner (--captioner ram); its tag list and per-class thresholds sit next to it (utils/caption.py)
+    "ram_plus": "ram_plus_swin_large_14m.pth",
 }
 UNSUPPORTED: Dict[str, str] = {}      # (every cleaner of the reference registry is built)
 

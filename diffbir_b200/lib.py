@@ -238,9 +238,32 @@ def layernorm(x, ldx, rows, c, gamma, beta, out, ldo, eps=1e-5, rows_per_group=0
     count_launch()
 
 
-def window_attention(qkv, ldq, batch, h, w, heads, head_dim, shift, bias_table, mask_value, out, ldo):
-    check(load().dbir_window_attention(_fp(qkv), C.c_int64(ldq), batch, h, w, heads, head_dim, 8, shift, _fp(bias_table),
-                                       C.c_float(mask_value), _fp(out), C.c_int64(ldo), _sp()), "dbir_window_attention")
+def window_attention(qkv, ldq, batch, h, w, heads, head_dim, shift, bias_table, mask_value, out, ldo, window=8):
+    check(load().dbir_window_attention(_fp(qkv), C.c_int64(ldq), batch, h, w, heads, head_dim, window, shift,
+                                       _fp(bias_table), C.c_float(mask_value), _fp(out), C.c_int64(ldo), _sp()),
+          "dbir_window_attention")
+    count_launch()
+
+
+def swin_patch_merge(x, ldx, n, h, w, c, gamma, beta, out, ldo, eps=1e-5):
+    """Swin PatchMerging gather + LayerNorm over 4c: fp32 x [n*h*w, ldx] -> op16 out [n*h/2*w/2, ldo]."""
+    check(load().dbir_swin_patch_merge(_fp(x), C.c_int64(ldx), n, h, w, c, _fp(gamma), _fp(beta), C.c_float(eps),
+                                       _fp(out), C.c_int64(ldo), _sp()), "dbir_swin_patch_merge")
+    count_launch()
+
+
+def token_mean(x, ldx, n, tokens, c, out, ldo):
+    """fp32 x [n*tokens, ldx] -> op16 out [n*(tokens+1), ldo]: per image [mean of its tokens | the tokens]."""
+    check(load().dbir_token_mean(_fp(x), C.c_int64(ldx), n, tokens, c, _fp(out), C.c_int64(ldo), _sp()),
+          "dbir_token_mean")
+    count_launch()
+
+
+def label_reweight(cls, ld_cls, batch, label_embed, classes, per_class, scale, out, ldo):
+    """RAM++ description reweighting: out[b*classes + k] = sum_j softmax_j(scale * cls_b/|cls_b| . e_kj) e_kj."""
+    check(load().dbir_label_reweight(_fp(cls), C.c_int64(ld_cls), batch, _fp(label_embed), classes, per_class,
+                                     label_embed.shape[-1], C.c_float(scale), _fp(out), C.c_int64(ldo), _sp()),
+          "dbir_label_reweight")
     count_launch()
 
 

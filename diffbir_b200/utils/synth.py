@@ -124,3 +124,13 @@ RUN_DEFAULTS = dict(steps=50, strength=1.0, cleaner_tiled=False, cleaner_tile_si
                     pos_prompt="", neg_prompt="low quality, blurry, low-resolution, noisy, unsharp, weird textures",
                     cfg_scale=4.0, start_point_type="noise", sampler_type="spaced", noise_aug=0,
                     rescale_cfg=False, s_churn=0, s_tmin=0, s_tmax=300, s_noise=1, eta=1, order=1)
+
+
+def synthetic_ram(seed: int = 1234):
+    """RAM++ with seeded weights (arch.ram_shapes) plus a generated tag list tag0000.. and seeded per-class thresholds
+    in [0.5, 1): (state_dict, tags, thresholds). Random weights give logits near 0, so the classes whose threshold
+    lies just above 0.5 are the ones that fire."""
+    from .. import arch
+    n = arch.RAM_CFG["num_class"]
+    thr = 0.5 + 0.5 * torch.rand(n, generator=_gen("ram_tag_list_threshold", seed))
+    return make_state_dict(arch.ram_shapes(arch.RAM_CFG), seed), [f"tag{i:04d}" for i in range(n)], thr.tolist()

@@ -105,7 +105,7 @@ int64_t dbir_attention_ws_bytes(int32_t batch, int32_t heads, int32_t sq, int32_
  * (unet.py:76-78, vae.py:37-40); do_norm = 0 gives a plain cast (operand of Down/Upsample
  * convs, 1x1 skip convs); out_raw (optional) receives the un-normalised cast.
  * dbir_layernorm: op16 out[rows, ldo] = LN(x[rows, c]) (attention.py:257-259,
- * swinir.py:208,214,722,783; eps 1e-5); columns [c, ldo) are zero-filled.
+ * swinir.py:208,214,722,783; eps 1e-5); columns [c, ldo) are zero-filled. c <= 1536 (ldo <= 1280 when c <= 1280).
  */
 int64_t dbir_gn_workspace_floats(int32_t n, int32_t hw, int32_t c);
 /* Per-(image, group) mean / rstd from the partial sums dbir_gemm emitted while writing the tensor(s)
@@ -141,8 +141,11 @@ int dbir_gn_merge(const double* moments, const int64_t* pixels, const int32_t* i
 /* imgs_per_group / rows_per_group > 0: stacked twin problems (see dbir_gemm_args.groups) -- image n /
  * row r takes gamma / beta at offset (n / imgs_per_group) * C resp. (r / rows_per_group) * c. 0 = one set. */
 
-/* ---- SwinIR / SCUNet window attention --------------------------------------------------
- * One 8x8 window per CTA; qkv op16 [batch*h*w, ldq] with columns [q | k | v] x (heads, dim)
+/* ---- SwinIR / SCUNet / Swin-L window attention -------------------------------------------
+ * window = 12 (RAM++'s Swin-L encoder, ram/models/swin_transformer.py:68-273): head_dim 32, any head count,
+ *   shift 0 or 6, h and w multiples of 12, ldq a multiple of 8 and qkv 16-byte aligned; tensor-core kernel, same
+ *   contract as below otherwise. window = 8: */
+/* One 8x8 window per CTA; qkv op16 [batch*h*w, ldq] with columns [q | k | v] x (heads, dim)
  * as produced by WindowAttention.qkv (swinir.py:104,122-123); out op16 [batch*h*w, ldo]
  * (first heads*dim columns) in original token order. shift = 0 (W-MSA) or 4 (SW-MSA):
  * replaces torch.roll + window_partition + q k^T + bias + mask + softmax + @v +
@@ -154,6 +157,23 @@ int dbir_gn_merge(const double* moments, const int64_t* pixels, const int32_t* i
 int dbir_window_attention(const void* qkv, int64_t ldq, int32_t batch, int32_t h, int32_t w, int32_t heads,
                           int32_t head_dim, int32_t window, int32_t shift, const float* bias_table, float mask_value,
                           void* out, int64_t ldo, void* stream);
+
+/* ---- RAM++ (ram/models/ram_plus.py) --------------------------------------------------------
+ * dbir_swin_patch_merge: PatchMerging (swin_transformer.py:294-331) up to its reduction GEMM: x fp32 [n*h*w, ldx]
+ *   (first c columns) -> op16 out[n*(h/2)*(w/2), ldo] = LN over 4c (gamma / beta fp32 [4c]) of the concat
+ *   [x(2i, 2j) | x(2i+1, 2j) | x(2i, 2j+1) | x(2i+1, 2j+1)].
+ * dbir_token_mean: x fp32 [n*tokens, ldx] -> op16 out[n*(tokens+1), ldo]: per image the mean of its tokens
+ *   (AdaptiveAvgPool1d, summed in token order) followed by the tokens themselves (swin_transformer.py:571-576).
+ * dbir_label_reweight: generate_tag's reweighting (ram_plus.py:291-309): for image b (cls row at cls + b*ld_cls,
+ *   dim = 512 floats) and class k, p = softmax_j(scale * cls/|cls| . e[k*per_class + j]) over per_class <= 64
+ *   descriptions of label_embed (op16 [classes*per_class, 512]), out row b*classes + k = sum_j p_j e_j (op16).
+ */
+int dbir_swin_patch_merge(const float* x, int64_t ldx, int32_t n, int32_t h, int32_t w, int32_t c, const float* gamma,
+                          const float* beta, float eps, void* out, int64_t ldo, void* stream);
+int dbir_token_mean(const float* x, int64_t ldx, int32_t n, int32_t tokens, int32_t c, void* out, int64_t ldo,
+                    void* stream);
+int dbir_label_reweight(const float* cls, int64_t ld_cls, int32_t batch, const void* label_embed, int32_t classes,
+                        int32_t per_class, int32_t dim, float scale, void* out, int64_t ldo, void* stream);
 
 /* ---- small / memory-bound ops ------------------------------------------------------------
  * conv3x3_small_cin : stems with <= 16 input channels; input = virtual concat of two NCHW
