@@ -5,4 +5,5 @@ from diffbir_b200.inference import (BFRInferenceLoop, BIDInferenceLoop, BSRInfer
 from .._unsupported import unsupported
 
 UnAlignedBFRInferenceLoop = unsupported("UnAlignedBFRInferenceLoop", "inference/unaligned_bfr_loop.py:14-152",
-                                        "face detection / alignment is outside the path; use BFRInferenceLoop on aligned faces")
+                                        "use diffbir_b200.inference.UnAlignedBFRInferenceLoop, or inference.py "
+                                        "--task unaligned_face")

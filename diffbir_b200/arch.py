@@ -531,3 +531,130 @@ def ram_state_dict(ckpt: dict, cfg: dict = None) -> dict:
         if tuple(sd[k].shape) != tuple(shp):
             raise ValueError(f"{k}: {tuple(sd[k].shape)} != {shp}")
     return sd
+
+
+# ---- face detector and face parser of the unaligned-face loop (facexlib 0.3 key layout) --------------------------
+RETINAFACE_CFG = dict(min_sizes=((16, 32), (64, 128), (256, 512)), steps=(8, 16, 32), variance=(0.1, 0.2),
+                      in_channel=256, out_channel=256, layers=(3, 4, 6, 3))
+PARSENET_CFG = dict(in_size=512, base_ch=64, min_feat_size=32, res_depth=10, parsing_ch=19, ch_range=(32, 256))
+BN_EPS = 1e-5
+
+
+def _bn(s: Shapes, p: str, c: int):
+    for nm in ("weight", "bias", "running_mean", "running_var"):
+        s[f"{p}.{nm}"] = (c,)
+
+
+def retinaface_shapes(cfg: dict = None) -> Shapes:
+    """RetinaFace(cfg_re50): `body.*` = torchvision resnet50 up to layer4 (stride on conv2), `fpn.output{1,2,3}` 1x1 and
+    `fpn.merge{1,2}` 3x3 conv + BN, `ssh{1,2,3}` conv + BN branches, then the per-level 1x1 heads."""
+    cfg = RETINAFACE_CFG if cfg is None else cfg
+    s = OrderedDict()
+    s["body.conv1.weight"] = (64, 3, 7, 7)
+    _bn(s, "body.bn1", 64)
+    cin = 64
+    for li, blocks in enumerate(cfg["layers"]):
+        w = 64 << li
+        for b in range(blocks):
+            p = f"body.layer{li + 1}.{b}."
+            s[p + "conv1.weight"] = (w, cin, 1, 1)
+            _bn(s, p + "bn1", w)
+            s[p + "conv2.weight"] = (w, w, 3, 3)
+            _bn(s, p + "bn2", w)
+            s[p + "conv3.weight"] = (4 * w, w, 1, 1)
+            _bn(s, p + "bn3", 4 * w)
+            if b == 0:
+                s[p + "downsample.0.weight"] = (4 * w, cin, 1, 1)
+                _bn(s, p + "downsample.1", 4 * w)
+            cin = 4 * w
+    ic, oc = cfg["in_channel"], cfg["out_channel"]
+    for i, c in enumerate((2 * ic, 4 * ic, 8 * ic)):
+        s[f"fpn.output{i + 1}.0.weight"] = (oc, c, 1, 1)
+        _bn(s, f"fpn.output{i + 1}.1", oc)
+    for i in (1, 2):
+        s[f"fpn.merge{i}.0.weight"] = (oc, oc, 3, 3)
+        _bn(s, f"fpn.merge{i}.1", oc)
+    for i in (1, 2, 3):
+        for nm, ci, co in (("conv3X3", oc, oc // 2), ("conv5X5_1", oc, oc // 4), ("conv5X5_2", oc // 4, oc // 4),
+                           ("conv7X7_2", oc // 4, oc // 4), ("conv7x7_3", oc // 4, oc // 4)):
+            s[f"ssh{i}.{nm}.0.weight"] = (co, ci, 3, 3)
+            _bn(s, f"ssh{i}.{nm}.1", co)
+    for head, k in (("ClassHead", 2), ("BboxHead", 4), ("LandmarkHead", 10)):
+        for i in range(3):
+            s[f"{head}.{i}.conv1x1.weight"] = (2 * k, oc, 1, 1)
+            s[f"{head}.{i}.conv1x1.bias"] = (2 * k,)
+    return s
+
+
+def parsenet_blocks(cfg: dict = None):
+    """(key prefix, cin, cout, scale) of every ResidualBlock of ParseNet(in_size=out_size=512), in forward order."""
+    cfg = PARSENET_CFG if cfg is None else cfg
+    lo, hi = cfg["ch_range"]
+    clip = lambda x: max(lo, min(x, hi))            # noqa: E731
+    steps = (cfg["in_size"] // min(cfg["in_size"], cfg["min_feat_size"])).bit_length() - 1
+    out, head = [], cfg["base_ch"]
+    for i in range(steps):
+        out.append((f"encoder.{i + 1}.", clip(head), clip(head * 2), "down"))
+        head *= 2
+    for i in range(cfg["res_depth"]):
+        out.append((f"body.{i}.", clip(head), clip(head), "none"))
+    for i in range(steps):
+        out.append((f"decoder.{i}.", clip(head), clip(head // 2), "up"))
+        head //= 2
+    return out
+
+
+def parsenet_shapes(cfg: dict = None) -> Shapes:
+    """ParseNet: ConvLayer keys `<p>conv2d.weight` (+ `.bias` without BN), BN under `<p>norm.norm.*`; a ResidualBlock
+    has `conv1`, `conv2` (BN) and, unless it keeps size and width, a `shortcut_func` conv (bias, no norm)."""
+    cfg = PARSENET_CFG if cfg is None else cfg
+    s = OrderedDict()
+    s["encoder.0.conv2d.weight"] = (cfg["base_ch"], 3, 3, 3)
+    s["encoder.0.conv2d.bias"] = (cfg["base_ch"],)
+    for p, ci, co, scale in parsenet_blocks(cfg):
+        if scale != "none" or ci != co:
+            s[p + "shortcut_func.conv2d.weight"] = (co, ci, 3, 3)
+            s[p + "shortcut_func.conv2d.bias"] = (co,)
+        s[p + "conv1.conv2d.weight"] = (co, ci, 3, 3)
+        _bn(s, p + "conv1.norm.norm", co)
+        s[p + "conv2.conv2d.weight"] = (co, co, 3, 3)
+        _bn(s, p + "conv2.norm.norm", co)
+    last = parsenet_blocks(cfg)[-1][2]
+    for nm, co in (("out_img_conv", 3), ("out_mask_conv", cfg["parsing_ch"])):
+        s[nm + ".conv2d.weight"] = (co, last, 3, 3)
+        s[nm + ".conv2d.bias"] = (co,)
+    return s
+
+
+def _strict(ckpt: dict, shapes: Shapes, what: str) -> dict:
+    if "state_dict" in ckpt and not hasattr(ckpt["state_dict"], "shape"):
+        ckpt = ckpt["state_dict"]
+    sd = {(k[len("module."):] if k.startswith("module.") else k): v for k, v in ckpt.items()
+          if not k.endswith("num_batches_tracked")}
+    missing = [k for k in shapes if k not in sd]
+    extra = [k for k in sd if k not in shapes]
+    bad = [f"{k} {tuple(sd[k].shape)} != {tuple(shapes[k])}" for k in shapes
+           if k in sd and tuple(sd[k].shape) != tuple(shapes[k])]
+    if missing or extra or bad:
+        raise ValueError(f"{what} checkpoint does not match: missing {missing}, unexpected {extra}, mis-shaped {bad}")
+    return sd
+
+
+def retinaface_state_dict(ckpt: dict, cfg: dict = None) -> dict:
+    """Strict loader of detection_Resnet50_Final.pth: `module.` stripped, num_batches_tracked ignored, every missing,
+    unexpected or mis-shaped key named."""
+    return _strict(ckpt, retinaface_shapes(cfg), "RetinaFace")
+
+
+def parsenet_state_dict(ckpt: dict, cfg: dict = None) -> dict:
+    """Strict loader of parsing_parsenet.pth (same rules as retinaface_state_dict)."""
+    return _strict(ckpt, parsenet_shapes(cfg), "ParseNet")
+
+
+def fold_bn(w, sd: dict, bn: str, bias=None, eps: float = BN_EPS):
+    """Eval-mode BatchNorm folded into the preceding conv, in fp32: (w * g / sqrt(var + eps), (b - mean) * that + beta)."""
+    import torch
+    scale = sd[bn + ".weight"].float() / torch.sqrt(sd[bn + ".running_var"].float() + eps)
+    b = torch.zeros_like(scale) if bias is None else bias.float()
+    return w.float() * scale.view(-1, *([1] * (w.dim() - 1))), (b - sd[bn + ".running_mean"].float()) * scale + \
+        sd[bn + ".bias"].float()

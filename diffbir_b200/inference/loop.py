@@ -230,10 +230,15 @@ class InferenceLoop:
             save_path = os.path.join(self.save_dir, file_name)
             Image.fromarray(sample).save(save_path)
             print(f"save result to {save_path}")
-        csv_path = os.path.join(self.save_dir, "prompt.csv")
-        new = not os.path.exists(csv_path)
-        with open(csv_path, "a", newline="") as f:
-            w = csv.writer(f)
-            if new:
-                w.writerow(["file_name", "pos_prompt", "neg_prompt"])
-            w.writerow([file_stem, pos_prompt, neg_prompt])
+        append_prompt_row(self.save_dir, file_stem, pos_prompt, neg_prompt)
+
+
+def append_prompt_row(save_dir: str, file_stem: str, pos_prompt: str, neg_prompt: str) -> None:
+    """One row of <save_dir>/prompt.csv, the header written with the first row."""
+    csv_path = os.path.join(save_dir, "prompt.csv")
+    new = not os.path.exists(csv_path)
+    with open(csv_path, "a", newline="") as f:
+        w = csv.writer(f)
+        if new:
+            w.writerow(["file_name", "pos_prompt", "neg_prompt"])
+        w.writerow([file_stem, pos_prompt, neg_prompt])

@@ -24,6 +24,9 @@ MODELS: Dict[str, str] = {
     "v2.1": "DiffBIR_v2.1.pt",
     # captioner (--captioner ram); its tag list and per-class thresholds sit next to it (utils/caption.py)
     "ram_plus": "ram_plus_swin_large_14m.pth",
+    # face detector and face parser of the unaligned-face loop (the files facexlib downloads)
+    "retinaface_resnet50": "detection_Resnet50_Final.pth",
+    "parsenet": "parsing_parsenet.pth",
 }
 UNSUPPORTED: Dict[str, str] = {}      # (every cleaner of the reference registry is built)
 

@@ -363,3 +363,49 @@ def wavelet_fix(sample, style, out_u8=None, out_f32=None):
                                   _fp(style), i64(style.stride(0)), i64(style.stride(1)), i64(style.stride(2)),
                                   b, h, w, _fp(out_u8), _fp(out_f32), _sp()), "dbir_wavelet_fix")
     count_launch()
+
+
+# ---- face detector / face parser (include/diffbir_b200.h, "face detector / face parser") ----
+def face_input(img_u8, n, h, w, out, *, scale=1.0, shift=(0.0, 0.0, 0.0), div=1.0, reverse=False):
+    check(load().dbir_face_input(_fp(img_u8), n, h, w, C.c_float(scale), C.c_float(shift[0]), C.c_float(shift[1]),
+                                 C.c_float(shift[2]), C.c_float(div), 1 if reverse else 0, _fp(out), _sp()),
+          "dbir_face_input")
+    count_launch()
+
+
+def patch_gather_shape(h, w, ksize, stride, up2=False):
+    """(ho, wo) of dbir_patch_gather's output grid."""
+    hs, ws, pad = (2 * h, 2 * w, ksize // 2) if up2 else (h, w, ksize // 2)
+    return (hs + 2 * pad - ksize) // stride + 1, (ws + 2 * pad - ksize) // stride + 1
+
+
+def patch_gather(x, ldx, n, h, w, c, ksize, stride, kpad, out, *, reflect=False, up2=False):
+    check(load().dbir_patch_gather(_fp(x), C.c_int64(ldx), n, h, w, c, ksize, stride, 1 if reflect else 0,
+                                   1 if up2 else 0, kpad, _fp(out), _sp()), "dbir_patch_gather")
+    count_launch()
+
+
+def maxpool3s2(x, n, h, w, c, out):
+    check(load().dbir_maxpool3s2(_fp(x), n, h, w, c, _fp(out), _sp()), "dbir_maxpool3s2")
+    count_launch()
+
+
+def fpn_add_up(a, b, n, h, w, hb, wb, c, out):
+    check(load().dbir_fpn_add_up(_fp(a), _fp(b), n, h, w, hb, wb, c, _fp(out), _sp()), "dbir_fpn_add_up")
+    count_launch()
+
+
+def relu_cast(x, numel, y16, y=None):
+    check(load().dbir_relu_cast(_fp(x), C.c_int64(numel), _fp(y), _fp(y16), _sp()), "dbir_relu_cast")
+    count_launch()
+
+
+def retinaface_decode(head, h, w, out):
+    check(load().dbir_retinaface_decode(_fp(head), h, w, _fp(out), _sp()), "dbir_retinaface_decode")
+    count_launch()
+
+
+def parse_mask(logits, ld, rows, classes, out):
+    check(load().dbir_parse_mask(_fp(logits), C.c_int64(ld), C.c_int64(rows), classes, _fp(out), _sp()),
+          "dbir_parse_mask")
+    count_launch()

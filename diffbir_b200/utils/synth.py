@@ -134,3 +134,32 @@ def synthetic_ram(seed: int = 1234):
     n = arch.RAM_CFG["num_class"]
     thr = 0.5 + 0.5 * torch.rand(n, generator=_gen("ram_tag_list_threshold", seed))
     return make_state_dict(arch.ram_shapes(arch.RAM_CFG), seed), [f"tag{i:04d}" for i in range(n)], thr.tolist()
+
+
+FACE_CLASS_GAIN = 15.0     # synthetic detector class heads: weight gain and face-logit bias (see synthetic_face_nets)
+FACE_CLASS_BIAS = -1.4
+
+
+def synthetic_face_nets(seed: int = 1234, class_gain: float = FACE_CLASS_GAIN, class_bias: float = FACE_CLASS_BIAS):
+    """Seeded RetinaFace-ResNet50 and ParseNet state dicts (arch.retinaface_shapes / parsenet_shapes).
+    - BatchNorm running variances are drawn in [1, 1.1): make_state_dict gives every norm shift 0.02 randn, and a
+      variance must be positive.
+    - The class heads' weights are scaled by `class_gain` and the face logits shifted by `class_bias`, so the score
+      spreads over priors and only the strongest few pass 0.8. On a 128x160 synthetic_lq input at x4 that is 1-4
+      faces, not none or thousands.
+    - The landmark heads' biases place the five points of every prior where the 512 FFHQ template has them within
+      a box of the prior's size, so detected faces have a plausible eye distance and alignment."""
+    from .face import FACE_TEMPLATE_512
+    from .. import arch
+    det = make_state_dict(arch.retinaface_shapes(), seed + 11)
+    parse = make_state_dict(arch.parsenet_shapes(), seed + 12)
+    for sd in (det, parse):
+        for k in sd:
+            if k.endswith("running_var"):
+                sd[k] = 1.0 + 0.1 * torch.rand(sd[k].shape, generator=_gen(k, seed))
+    lm = torch.tensor(((FACE_TEMPLATE_512 - 256.0) / 512.0 / 0.1).reshape(-1), dtype=torch.float32)
+    for i in range(3):
+        det[f"ClassHead.{i}.conv1x1.weight"] *= class_gain
+        det[f"ClassHead.{i}.conv1x1.bias"][1::2] += class_bias
+        det[f"LandmarkHead.{i}.conv1x1.bias"] += torch.cat([lm, lm])
+    return det, parse

@@ -175,6 +175,34 @@ int dbir_token_mean(const float* x, int64_t ldx, int32_t n, int32_t tokens, int3
 int dbir_label_reweight(const float* cls, int64_t ld_cls, int32_t batch, const void* label_embed, int32_t classes,
                         int32_t per_class, int32_t dim, float scale, void* out, int64_t ldo, void* stream);
 
+/* ---- face detector / face parser (unaligned-face loop; facexlib RetinaFace-ResNet50 and ParseNet) -----------------
+ * dbir_face_input: uint8 HWC pixels [n*h*w, 3] -> op16 [n*h*w, 3], out[c] = (src[c'] * scale - shift_c) / div with
+ *   c' = 2 - c when reverse (RetinaFace: minus (104, 117, 123); ParseNet: img2tensor's channel swap, (x/255 - .5)/.5).
+ * dbir_patch_gather: patch matrix of a ksize x ksize (1, 3, 7) convolution with stride 1 or 2, pad ksize/2 (zeros, or
+ *   reflection when reflect = 1), optionally on the nearest-2x up-sampled input (up2 = 1): op16 x NHWC [n, h, w, ldx]
+ *   (first c channels) -> op16 out [n*ho*wo, kpad], column tap*c + ch (taps row-major), columns >= ksize^2 c zero;
+ *   kpad a multiple of 64. Feeds dbir_gemm's matrix mode for the convolutions its conv mode does not take.
+ * dbir_maxpool3s2: 3x3 / stride 2 / pad 1 max pool, op16 NHWC, c % 8 == 0 (resnet50 stem).
+ * dbir_fpn_add_up: op16 out = a + F.interpolate(b, size=(h, w), mode="nearest") with PyTorch's index rule; a fp32
+ *   NHWC [n, h, w, c], b op16 NHWC [n, hb, wb, c].
+ * dbir_relu_cast: y = relu(x) (fp32, y may be x or NULL) and its op16 copy y16; x = conv + identity (bottleneck tail).
+ * dbir_retinaface_decode: head fp32 [rows, 32] (per pixel of the three levels, back to back: class logits 2x2 | box
+ *   2x4 | landmarks 2x10) of an h x w input -> out fp32 [2 rows, 15] = x1 y1 x2 y2 score l1x l1y .. l5x l5y per prior
+ *   (PriorBox order, min sizes 16/32, 64/128, 256/512, steps 8/16/32, variances 0.1/0.2), in input pixels.
+ * dbir_parse_mask: per row of fp32 logits [rows, ld], argmax over `classes` (first maximum) -> uint8 255 for the
+ *   face classes of FaceRestoreHelper's colormap (1-13, 15), else 0.
+ */
+int dbir_face_input(const uint8_t* img, int32_t n, int32_t h, int32_t w, float scale, float shift0, float shift1,
+                    float shift2, float div, int32_t reverse, void* out, void* stream);
+int dbir_patch_gather(const void* x, int64_t ldx, int32_t n, int32_t h, int32_t w, int32_t c, int32_t ksize,
+                      int32_t stride, int32_t reflect, int32_t up2, int32_t kpad, void* out, void* stream);
+int dbir_maxpool3s2(const void* x, int32_t n, int32_t h, int32_t w, int32_t c, void* out, void* stream);
+int dbir_fpn_add_up(const float* a, const void* b, int32_t n, int32_t h, int32_t w, int32_t hb, int32_t wb, int32_t c,
+                    void* out, void* stream);
+int dbir_relu_cast(const float* x, int64_t numel, float* y, void* y16, void* stream);
+int dbir_retinaface_decode(const float* head, int32_t h, int32_t w, float* out, void* stream);
+int dbir_parse_mask(const float* logits, int64_t ld, int64_t rows, int32_t classes, uint8_t* out, void* stream);
+
 /* ---- small / memory-bound ops ------------------------------------------------------------
  * conv3x3_small_cin : stems with <= 16 input channels; input = virtual concat of two NCHW
  *   fp32 tensors scaled by in_scale/in_shift; weight fp32 [9*Cin, Cout]; out NHWC fp32

@@ -103,13 +103,12 @@ def main(argv=None) -> None:
     if args.device == "cuda" and not torch.cuda.is_available():
         raise SystemExit("inference.py needs a CUDA device (sm_90a): there is no CPU fallback for the engines")
     set_seed(args.seed)
-    from diffbir_b200.inference import BFRInferenceLoop, BIDInferenceLoop, BSRInferenceLoop, CustomInferenceLoop
-    loops = {"sr": BSRInferenceLoop, "face": BFRInferenceLoop, "denoise": BIDInferenceLoop}
+    from diffbir_b200.inference import (BFRInferenceLoop, BIDInferenceLoop, BSRInferenceLoop, CustomInferenceLoop,
+                                        UnAlignedBFRInferenceLoop)
+    loops = {"sr": BSRInferenceLoop, "face": BFRInferenceLoop, "denoise": BIDInferenceLoop,
+             "unaligned_face": UnAlignedBFRInferenceLoop}
     if args.version == "custom":
         CustomInferenceLoop(args).run()
-    elif args.task not in loops:
-        raise NotImplementedError(f"--task {args.task}: the unaligned-face loop needs the face detector, which is outside "
-                                  "the accelerated path (SURVEY.md §8f)")
     else:
         loops[args.task](args).run()
     print("done!")
