@@ -658,3 +658,113 @@ def fold_bn(w, sd: dict, bn: str, bias=None, eps: float = BN_EPS):
     b = torch.zeros_like(scale) if bias is None else bias.float()
     return w.float() * scale.view(-1, *([1] * (w.dim() - 1))), (b - sd[bn + ".running_mean"].float()) * scale + \
         sd[bn + ".bias"].float()
+
+
+# ---- LLaVA-1.5-7B captioner (reference utils/caption.py:52-145, llava/model/*) --------------------------------------
+# LLM: LLaMA-7B (Vicuna-7B v1.5); vision tower: CLIP ViT-L/14-336; projector mlp2x_gelu. Keys in the layout of the
+# llava-v1.5-7b shards, the vision tower under model.vision_tower.vision_tower.vision_model.* (CLIPVisionTower).
+LLAVA_CFG = dict(vocab=32000, hidden=4096, layers=32, heads=32, intermediate=11008, rms_eps=1e-5, rope_theta=10000.0,
+                 bos=1, eos=2, image=336, patch=14, v_width=1024, v_layers=24, v_heads=16, v_intermediate=4096,
+                 v_eps=1e-5, select_layer=-2)
+LLAVA_HEAD_DIM = 128
+VISION_PREFIX = "model.vision_tower.vision_tower."
+
+
+def llava_config(config: dict, clip_config: Optional[dict] = None) -> dict:
+    """Sizes from llava-v1.5-7b's config.json (and the CLIP directory's config.json, if any). Anything but the v1.5
+    settings the engine implements is refused with a message naming the setting."""
+    def need(key, want, ok):
+        got = config.get(key, want)
+        if not ok(got):
+            raise NotImplementedError(f"LLaVA config.json: {key} = {got!r}; only {want!r} (LLaVA-1.5) is built")
+    need("mm_projector_type", "mlp2x_gelu", lambda v: v == "mlp2x_gelu")
+    need("image_aspect_ratio", "pad", lambda v: v == "pad")
+    need("mm_vision_select_layer", -2, lambda v: v == -2)
+    need("mm_vision_select_feature", "patch", lambda v: v == "patch")
+    need("mm_use_im_start_end", False, lambda v: not v)
+    need("rope_scaling", None, lambda v: v is None)
+    heads = config["num_attention_heads"]
+    need("num_key_value_heads", heads, lambda v: v == heads)
+    if config["hidden_size"] != heads * LLAVA_HEAD_DIM:
+        raise NotImplementedError(f"LLaVA config.json: hidden_size {config['hidden_size']} != {heads} heads x 128")
+    cfg = dict(LLAVA_CFG, vocab=config["vocab_size"], hidden=config["hidden_size"], layers=config["num_hidden_layers"],
+               heads=heads, intermediate=config["intermediate_size"], rms_eps=config.get("rms_norm_eps", 1e-5),
+               rope_theta=float(config.get("rope_theta", 10000.0)), bos=config.get("bos_token_id", 1),
+               eos=config.get("eos_token_id", 2))
+    if "mm_hidden_size" in config:
+        cfg["v_width"] = config["mm_hidden_size"]
+    if clip_config is not None:
+        v = clip_config.get("vision_config", clip_config)
+        if v.get("hidden_act", "quick_gelu") != "quick_gelu":
+            raise NotImplementedError(f"CLIP config.json: hidden_act {v['hidden_act']!r}; only quick_gelu is built")
+        cfg.update(image=v.get("image_size", 336), patch=v.get("patch_size", 14), v_width=v["hidden_size"],
+                   v_layers=v["num_hidden_layers"], v_heads=v["num_attention_heads"],
+                   v_intermediate=v["intermediate_size"], v_eps=v.get("layer_norm_eps", 1e-5))
+    return cfg
+
+
+def llava_shapes(cfg: dict) -> Shapes:
+    s: Shapes = OrderedDict()
+    d, f, vw = cfg["hidden"], cfg["intermediate"], cfg["v_width"]
+    s["model.embed_tokens.weight"] = (cfg["vocab"], d)
+    for i in range(cfg["layers"]):
+        p = f"model.layers.{i}."
+        for nm in ("q_proj", "k_proj", "v_proj", "o_proj"):
+            s[p + f"self_attn.{nm}.weight"] = (d, d)
+        s[p + "mlp.gate_proj.weight"] = (f, d)
+        s[p + "mlp.up_proj.weight"] = (f, d)
+        s[p + "mlp.down_proj.weight"] = (d, f)
+        s[p + "input_layernorm.weight"] = (d,)
+        s[p + "post_attention_layernorm.weight"] = (d,)
+    s["model.norm.weight"] = (d,)
+    s["lm_head.weight"] = (cfg["vocab"], d)
+    s["model.mm_projector.0.weight"] = (d, vw)
+    s["model.mm_projector.0.bias"] = (d,)
+    s["model.mm_projector.2.weight"] = (d, d)
+    s["model.mm_projector.2.bias"] = (d,)
+    v = VISION_PREFIX + "vision_model."
+    side = cfg["image"] // cfg["patch"]
+    s[v + "embeddings.class_embedding"] = (vw,)
+    s[v + "embeddings.patch_embedding.weight"] = (vw, 3, cfg["patch"], cfg["patch"])
+    s[v + "embeddings.position_embedding.weight"] = (side * side + 1, vw)
+    s[v + "pre_layrnorm.weight"] = (vw,)
+    s[v + "pre_layrnorm.bias"] = (vw,)
+    for i in range(cfg["v_layers"]):
+        p = f"{v}encoder.layers.{i}."
+        for nm in ("q_proj", "k_proj", "v_proj", "out_proj"):
+            s[p + f"self_attn.{nm}.weight"] = (vw, vw)
+            s[p + f"self_attn.{nm}.bias"] = (vw,)
+        for nm in ("layer_norm1", "layer_norm2"):
+            s[p + nm + ".weight"] = (vw,)
+            s[p + nm + ".bias"] = (vw,)
+        s[p + "mlp.fc1.weight"] = (cfg["v_intermediate"], vw)
+        s[p + "mlp.fc1.bias"] = (cfg["v_intermediate"],)
+        s[p + "mlp.fc2.weight"] = (vw, cfg["v_intermediate"])
+        s[p + "mlp.fc2.bias"] = (vw,)
+    s[v + "post_layernorm.weight"] = (vw,)
+    s[v + "post_layernorm.bias"] = (vw,)
+    return s
+
+
+def llava_state_dict(llava_sd: dict, clip_sd: Optional[dict] = None, cfg: dict = None) -> dict:
+    """The strict LLaVA loader. llava_sd: the merged llava-v1.5-7b shards; clip_sd: the CLIP ViT-L/14-336 checkpoint
+    (its vision_model.* keys become the vision tower; the text tower and projections it also holds are not used), or
+    None when the shards carry model.vision_tower.*. Buffers the checkpoints may hold (rotary inv_freq, position_ids)
+    are dropped; every other key must be one of llava_shapes, with its shape."""
+    cfg = LLAVA_CFG if cfg is None else cfg
+    buffers = ("rotary_emb.inv_freq", "position_ids")
+    sd = {k: v for k, v in llava_sd.items() if not k.endswith(buffers)}
+    if clip_sd is not None:
+        if any(k.startswith("model.vision_tower.") for k in sd):
+            raise ValueError("LLaVA checkpoint carries model.vision_tower.* and a CLIP checkpoint was given too")
+        sd.update({VISION_PREFIX + k: v for k, v in clip_sd.items()
+                   if k.startswith("vision_model.") and not k.endswith(buffers)})
+    shapes = llava_shapes(cfg)
+    missing = [k for k in shapes if k not in sd]
+    extra = [k for k in sd if k not in shapes]
+    bad = [f"{k} {tuple(sd[k].shape)} != {tuple(shapes[k])}" for k in shapes
+           if k in sd and tuple(sd[k].shape) != tuple(shapes[k])]
+    if missing or extra or bad:
+        raise ValueError(f"LLaVA checkpoint does not match: missing {missing[:8]}{' ...' if len(missing) > 8 else ''}, "
+                         f"unexpected {extra[:8]}{' ...' if len(extra) > 8 else ''}, mis-shaped {bad[:8]}")
+    return sd

@@ -25,6 +25,7 @@
 #include <array>
 #include <map>
 #include <mutex>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -52,9 +53,10 @@ struct GemmParams {
   int rows_per_vec;
   int has_residual;
   float alpha;
-  int act;                 // 0 none, 1 gelu(erf), 2 leaky relu (slope in act_param), 3 silu
+  int act;                 // 0 none, 1 gelu(erf), 2 leaky relu (slope in act_param), 3 silu, 4 quick_gelu
   float act_param;
-  int geglu;               // 1: tile holds [BN/2 values | BN/2 gates]; output width N/2
+  int geglu;               // 1: tile holds [BN/2 values | BN/2 gates], out = values * gelu(gates); 2: the same
+                           // packing, out = values * silu(gates) (SwiGLU); output width N/2
   int bias_per_row;        // bias indexed by output row instead of column
   // grouped launch: G same-shape problems back to back along M; group g's weights / bias start at row g*N
   int group_span;          // m-tiles (plain) or images (conv) per group; 0 = one problem
@@ -72,7 +74,8 @@ struct GemmParams {
 __device__ __forceinline__ float apply_act(float v, int act, float prm) {
   if (act == 1) return gelu_erf_f(v);
   if (act == 2) return v > 0.f ? v : v * prm;
-  return silu_f(v);
+  // 3: silu x * sigmoid(x), 4: quick_gelu x * sigmoid(1.702 x) (CLIP MLP); -1.0f * v == -v, so silu is unchanged
+  return v / (1.0f + __expf((act == 4 ? -1.702f : -1.0f) * v));
 }
 
 __device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
@@ -615,18 +618,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
           asm volatile("st.shared.f32 [%0], %1;" ::"r"(bb + (i * 64 + 32 + lane) * 4), "f"(pg[i]) : "memory");
         }
         __syncwarp();
-        int ci = 0;
-#pragma unroll
-        for (int i = 0; i < MAX_G; ++i) {
+        // one chunk of values * act(gates); false once the chunks of this warp are done. SWIGLU (geglu = 2) runs
+        // as a rolled loop so that the GEGLU path keeps its code unchanged.
+        auto chunk = [&](int i, int& ci, auto swiglu) -> bool {
           const int c0 = c_first + i * CSTEP;
-          if (c0 >= HB) break;
+          if (c0 >= HB) return false;
           float av[32], ag[32];
           e.cur = acc_block(acc_base, c0 >> 5, q);
           __syncwarp();
           acc_ld32(e.cur, lane, av);
           acc_ld32(acc_block(acc_base, (HB + c0) >> 5, q), lane, ag);
           const int gc0 = n_tile * HB + c0;   // output column
-          if (gc0 >= n_half) continue;
+          if (gc0 >= n_half) return true;
           const int ncols = min(32, n_half - gc0);
           float v[32];
 #pragma unroll
@@ -637,13 +640,28 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant_
             fadd2(a2, a3, av[4 * jj + 2], av[4 * jj + 3], ba.z, ba.w);
             fadd2(g0, g1, ag[4 * jj], ag[4 * jj + 1], bg.x, bg.y);
             fadd2(g2, g3, ag[4 * jj + 2], ag[4 * jj + 3], bg.z, bg.w);
-            gelu_erf_f2(g0, g1, y0, y1);
-            gelu_erf_f2(g2, g3, y2, y3);
+            if constexpr (decltype(swiglu)::value) {
+              y0 = silu_f(g0); y1 = silu_f(g1); y2 = silu_f(g2); y3 = silu_f(g3);
+            } else {
+              gelu_erf_f2(g0, g1, y0, y1);
+              gelu_erf_f2(g2, g3, y2, y3);
+            }
             fmul2(v[4 * jj], v[4 * jj + 1], a0, a1, y0, y1);
             fmul2(v[4 * jj + 2], v[4 * jj + 3], a2, a3, y2, y3);
           }
           finish_chunk(p, e, v, lane, ci, gc0, ncols, -1, out_row, vec_idx, false);
           ++ci;
+          return true;
+        };
+        int ci = 0;
+        if (p.geglu == 2) {
+#pragma unroll 1
+          for (int i = 0; i < MAX_G; ++i)
+            if (!chunk(i, ci, std::true_type{})) break;
+        } else {
+#pragma unroll
+          for (int i = 0; i < MAX_G; ++i)
+            if (!chunk(i, ci, std::false_type{})) break;
         }
       }
     }

@@ -86,7 +86,10 @@ def check_supported(args: Namespace) -> None:
         raise NotImplementedError(f"--device {args.device}: the engines are CUDA (sm_90a) only, there is no CPU path")
     if args.sampler not in SUPPORTED_SAMPLERS:
         raise NotImplementedError(f"--sampler {args.sampler}: not one of {SUPPORTED_SAMPLERS}")
-    if args.captioner not in ("none", "ram"):
+    if args.captioner == "llava" and str(getattr(args, "llava_bit", "4")) != "16":
+        from ..utils.caption import llava_bit_message
+        raise NotImplementedError(llava_bit_message(getattr(args, "llava_bit", "4")))
+    if args.captioner not in ("none", "ram", "llava"):
         raise NotImplementedError(f"--captioner {args.captioner}: captioners are outside the path; pass --captioner none "
                                   "and a --pos_prompt")
     if args.guidance:
@@ -128,8 +131,13 @@ class InferenceLoop:
         raise NotImplementedError
 
     def load_captioner(self) -> None:
-        """loop.py:119-129: --captioner none -> no caption, ram -> RAM++ tags on the engine."""
-        if self.args.captioner == "ram":
+        """loop.py:119-129: --captioner none -> no caption, ram -> RAM++ tags, llava -> a LLaVA-1.5 description, each
+        on the engine."""
+        if self.args.captioner == "llava":
+            from ..utils.caption import LLaVACaptioner
+            self.captioner = LLaVACaptioner(self.args.device, self.args.llava_bit, self.weights_dir, self.synthetic,
+                                            self.args.seed)
+        elif self.args.captioner == "ram":
             from ..utils.caption import RAMCaptioner
             self.captioner = RAMCaptioner(self.args.device, self.weights_dir, self.synthetic, self.args.seed)
         else:

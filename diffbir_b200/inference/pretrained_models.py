@@ -27,7 +27,12 @@ MODELS: Dict[str, str] = {
     # face detector and face parser of the unaligned-face loop (the files facexlib downloads)
     "retinaface_resnet50": "detection_Resnet50_Final.pth",
     "parsenet": "parsing_parsenet.pth",
+    # --captioner llava --llava_bit 16: directories in the Hugging Face layouts the reference loads
+    # (liuhaotian/llava-v1.5-7b and its vision tower openai/clip-vit-large-patch14-336)
+    "llava_v1.5_7b": "llava-v1.5-7b",
+    "clip_vit_l14_336": "clip-vit-large-patch14-336",
 }
+DIRECTORIES = {"llava_v1.5_7b", "clip_vit_l14_336"}     # keys that name a directory, not a file
 UNSUPPORTED: Dict[str, str] = {}      # (every cleaner of the reference registry is built)
 
 
@@ -39,6 +44,13 @@ def resolve(key: str, weights_dir: str) -> str:
     if key in UNSUPPORTED:
         raise NotImplementedError(f"checkpoint '{key}' belongs to a cleaner outside the accelerated path")
     path = os.path.join(weights_dir, MODELS[key])
+    if key in DIRECTORIES:
+        if not os.path.isdir(path):
+            raise FileNotFoundError(
+                f"model directory '{key}' not found at {path}: place the Hugging Face directory {MODELS[key]} "
+                "(config.json, tokenizer / checkpoint shards) in --weights_dir (no network access here), or pass "
+                "--synthetic")
+        return path
     if not os.path.isfile(path):
         raise FileNotFoundError(
             f"checkpoint '{key}' not found at {path}: place the file the reference downloads for this key "

@@ -104,14 +104,15 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
-ACT = {None: 0, "none": 0, "gelu": 1, "lrelu": 2, "silu": 3}
+ACT = {None: 0, "none": 0, "gelu": 1, "lrelu": 2, "silu": 3, "quick_gelu": 4}
 
 
 def gemm(a, b, out, *, M, N, K, bias=None, rowvec=None, rows_per_vec=0, residual=None,
          lda=0, ldb=0, ldo=None, ldr=None, conv=None, act=None, act_param=0.0, alpha=1.0,
          geglu=False, force_bn=0, bias_per_row=False, splitk_ws=None, split_k=0, cta_pair=0,
          gn_partials=None, gn_rows_per_img=0, groups=1):
-    """out = residual + alpha * act(A @ B^T + bias + rowvec). conv = (n, h, w, c, ksize)."""
+    """out = residual + alpha * act(A @ B^T + bias + rowvec). conv = (n, h, w, c, ksize).
+    geglu: False / True (= 1, values * gelu(gates)) or 2 (values * silu(gates)), weights packed per force_bn tile."""
     lib = load()
     g = GemmArgs()
     g.a, g.b, g.out = a.data_ptr(), b.data_ptr(), out.data_ptr()
@@ -131,7 +132,7 @@ def gemm(a, b, out, *, M, N, K, bias=None, rowvec=None, rows_per_vec=0, residual
     g.act = ACT[act]
     g.act_param = act_param
     g.alpha = alpha
-    g.geglu = 1 if geglu else 0
+    g.geglu = int(geglu)
     g.force_bn = force_bn
     g.bias_per_row = 1 if bias_per_row else 0
     g.groups = groups
@@ -408,4 +409,60 @@ def retinaface_decode(head, h, w, out):
 def parse_mask(logits, ld, rows, classes, out):
     check(load().dbir_parse_mask(_fp(logits), C.c_int64(ld), C.c_int64(rows), classes, _fp(out), _sp()),
           "dbir_parse_mask")
+    count_launch()
+
+
+# ---- LLaVA captioner language model (include/diffbir_b200.h, "LLaVA captioner language model") ----
+def rmsnorm(x, ldx, rows, c, w, out, ldo, eps=1e-5):
+    check(load().dbir_rmsnorm(_fp(x), C.c_int64(ldx), rows, c, _fp(w), C.c_float(eps), _fp(out), C.c_int64(ldo), _sp()),
+          "dbir_rmsnorm")
+    count_launch()
+
+
+def rope_kv(qkv, ldqkv, rows, heads, p0, q, ldq, k_cache, v_cache, theta=10000.0):
+    check(load().dbir_rope_kv(_fp(qkv), C.c_int64(ldqkv), rows, heads, _fp(p0), C.c_float(theta), _fp(q), C.c_int64(ldq),
+                              _fp(k_cache), _fp(v_cache), _sp()), "dbir_rope_kv")
+    count_launch()
+
+
+def attention_causal(q, ldq, k_cache, v_cache, heads, sq, out, ldo):
+    check(load().dbir_attention_causal(_fp(q), C.c_int64(ldq), _fp(k_cache), _fp(v_cache), heads, sq, _fp(out),
+                                       C.c_int64(ldo), _sp()), "dbir_attention_causal")
+    count_launch()
+
+
+def attention_decode_ws_bytes(heads, capacity) -> int:
+    lib = load()
+    lib.dbir_attention_decode_ws_bytes.restype = C.c_int64
+    return int(lib.dbir_attention_decode_ws_bytes(heads, capacity))
+
+
+def attention_decode(q, k_cache, v_cache, heads, capacity, length, ws, out):
+    """length: device int32 [1] holding the number of cache rows to attend to."""
+    check(load().dbir_attention_decode(_fp(q), _fp(k_cache), _fp(v_cache), heads, capacity, _fp(length), _fp(ws),
+                                       C.c_int64(ws.numel() * ws.element_size()), _fp(out), _sp()),
+          "dbir_attention_decode")
+    count_launch(2)
+
+
+GEMV_EPILOGUE = {"none": 0, "residual": 1, "swiglu": 2}
+
+
+def gemv(w, x, y, *, N, K, ldw=0, epilogue="none", pack=0, residual=None):
+    """y = W x for one row (op16 W [N, ldw], op16 x [K]); y fp32 or op16. epilogue: none / residual / swiglu."""
+    check(load().dbir_gemv(_fp(w), C.c_int64(ldw or K), _fp(x), N, K, GEMV_EPILOGUE[epilogue], pack, _fp(residual),
+                           _fp(y), 0 if y.dtype == torch.float32 else 1, _sp()), "dbir_gemv")
+    count_launch()
+
+
+def argmax(logits, n, token, advance=None):
+    """First maximum of fp32 logits [n] -> device int32 token; each element of `advance` (device int32) += 1."""
+    n_adv = 0 if advance is None else advance.numel()
+    check(load().dbir_argmax(_fp(logits), n, _fp(token), _fp(advance), n_adv, _sp()), "dbir_argmax")
+    count_launch()
+
+
+def embed_gather(table, vocab, ids, n, dim, out, ldo):
+    check(load().dbir_embed_gather(_fp(table), vocab, _fp(ids), n, dim, _fp(out), C.c_int64(ldo), _sp()),
+          "dbir_embed_gather")
     count_launch()

@@ -163,3 +163,30 @@ def synthetic_face_nets(seed: int = 1234, class_gain: float = FACE_CLASS_GAIN, c
         det[f"ClassHead.{i}.conv1x1.bias"][1::2] += class_bias
         det[f"LandmarkHead.{i}.conv1x1.bias"] += torch.cat([lm, lm])
     return det, parse
+
+
+def synthetic_llava(cfg: dict, seed: int = 1234, device="cuda", lm_head_scale: float = 1.0):
+    """LLaVA-1.5 weights (arch.llava_shapes of cfg) drawn on `device` with the distributions of make_state_dict: at
+    the 7B size a host generator would take minutes. Matrices are stored in fp16 (the checkpoints' dtype), vectors in
+    fp32; each tensor has its own seeded device generator. lm_head is multiplied by lm_head_scale."""
+    from .. import arch
+    sd = OrderedDict()
+    for key, shape in arch.llava_shapes(cfg).items():
+        g = torch.Generator(device=device)
+        g.manual_seed((zlib.crc32(key.encode()) ^ (seed * 0x9E3779B1)) & 0x7FFFFFFF)
+        if len(shape) >= 2:
+            fan_in = 1
+            for d in shape[1:]:
+                fan_in *= d
+            if "embed" in key:
+                t = torch.randn(shape, generator=g, device=device, dtype=torch.float16) * 0.02
+            else:
+                t = torch.rand(shape, generator=g, device=device, dtype=torch.float16).mul_(2).sub_(1).mul_(fan_in ** -0.5)
+            if key == "lm_head.weight":
+                t.mul_(lm_head_scale)
+        elif key.endswith("weight"):
+            t = 1.0 + 0.05 * torch.randn(shape, generator=g, device=device)
+        else:
+            t = 0.02 * torch.randn(shape, generator=g, device=device)
+        sd[key] = t
+    return sd

@@ -48,8 +48,11 @@ typedef struct dbir_gemm_args {
   int32_t img_n, img_h, img_w, img_c, ksize;
   int32_t rows_per_vec; /* a_mode 0 only; conv mode uses the image index */
   int32_t out_kind;     /* 0 fp32, 1 op16 */
-  int32_t act;          /* 0 none, 1 GELU(erf), 2 LeakyReLU(act_param), 3 SiLU */
-  int32_t geglu;        /* 1: B rows packed per force_bn-row tile as [values | gates]; out has N/2 columns */
+  int32_t act;          /* 0 none, 1 GELU(erf), 2 LeakyReLU(act_param), 3 SiLU, 4 quick_gelu x * sigmoid(1.702 x)
+                           (CLIP MLP, clip_encoder.py -> CLIPMLP with hidden_act "quick_gelu") */
+  int32_t geglu;        /* B rows packed per force_bn-row tile as [values | gates]; out has N/2 columns:
+                           1 = values * gelu(gates) (GEGLU), 2 = values * silu(gates) (LLaMA's SwiGLU MLP,
+                           down_proj(act(gate_proj(x)) * up_proj(x)) with values = up, gates = gate) */
   int32_t force_bn;     /* 0 = auto tile width, else 32/64/128/160/256 (required with geglu) */
   float alpha;          /* scale applied before the residual add (control strength) */
   float act_param;
@@ -202,6 +205,43 @@ int dbir_fpn_add_up(const float* a, const void* b, int32_t n, int32_t h, int32_t
 int dbir_relu_cast(const float* x, int64_t numel, float* y, void* y16, void* stream);
 int dbir_retinaface_decode(const float* head, int32_t h, int32_t w, float* out, void* stream);
 int dbir_parse_mask(const float* logits, int64_t ld, int64_t rows, int32_t classes, uint8_t* out, void* stream);
+
+/* ---- LLaVA captioner language model (LLaMA-7B, transformers' modeling_llama.py as loaded by the reference's
+ * llava/model/language_model/llava_llama.py; decode loop = LlavaLlamaForCausalLM.generate in utils/caption.py:52-145)
+ * Every length or position that changes per generated token is a DEVICE int32 scalar, so one captured decode graph
+ * replays for every token. KV caches are op16 [capacity, heads, 128].
+ * dbir_rmsnorm: LlamaRMSNorm: op16 out[r] = w * x[r] / sqrt(mean(x[r]^2) + eps) over c fp32 columns (per-layer
+ *   input_layernorm / post_attention_layernorm and the final norm). c, ldx, ldo multiples of 4.
+ * dbir_rope_kv: rows of the fused QKV product (fp32 [rows, ldqkv], columns [q | k | v] x heads x 128) at positions
+ *   p0[0] + i: rotary embedding (apply_rotary_pos_emb, rotate_half form, inv_freq = theta^(-2j/128)) of q and k in
+ *   fp32; q -> op16 [rows, ldq], k and v -> the caches at row p0[0] + i (LlamaAttention + DynamicCache.update).
+ * dbir_attention_causal: prefill: queries q op16 [sq, ldq] at positions 0 .. sq-1 against cache rows 0 .. sq-1,
+ *   causal, scale 128^-0.5, tensor cores (mma.sync) -> op16 out [sq, ldo] (LlamaAttention with the causal mask).
+ * dbir_attention_decode: one query row per head (q op16 [heads*128]) against cache rows 0 .. len[0]-1
+ *   (1 <= len[0] <= capacity), split over 64-key chunks, combined in chunk order (deterministic) -> op16 out
+ *   [heads*128]. ws: dbir_attention_decode_ws_bytes(heads, capacity) bytes, no initialisation needed.
+ * dbir_gemv: y = W x for one row: W op16 [N, ldw] (K contiguous: the packed weight dbir_gemm reads), x op16 [K],
+ *   fp32 accumulation. epilogue 0: y = Wx (QKV, lm_head); 1: y = Wx + residual (fp32 [N]; y may be the residual:
+ *   o_proj, down_proj); 2: SwiGLU over rows packed per `pack`-row tile as [values | gates] (dbir_gemm's geglu 2
+ *   packing with force_bn = pack): y[c] = values . x * silu(gates . x), N/2 outputs. out_kind 0 fp32, 1 op16.
+ * dbir_argmax: first maximum of fp32 logits [n] -> *token (greedy decoding, temperature 0); then each of
+ *   advance[0 .. n_advance-1] (device int32) is incremented by one: the decode step's position and length.
+ * dbir_embed_gather: fp32 out[i, ldo] = embed_tokens[ids[i]] (op16 [vocab, dim]; ids device int32 [n]).
+ */
+int dbir_rmsnorm(const float* x, int64_t ldx, int32_t rows, int32_t c, const float* w, float eps, void* out, int64_t ldo,
+                 void* stream);
+int dbir_rope_kv(const float* qkv, int64_t ldqkv, int32_t rows, int32_t heads, const int32_t* p0, float theta, void* q,
+                 int64_t ldq, void* k_cache, void* v_cache, void* stream);
+int dbir_attention_causal(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int32_t heads, int32_t sq,
+                          void* out, int64_t ldo, void* stream);
+int64_t dbir_attention_decode_ws_bytes(int32_t heads, int32_t capacity);
+int dbir_attention_decode(const void* q, const void* k_cache, const void* v_cache, int32_t heads, int32_t capacity,
+                          const int32_t* len, void* ws, int64_t ws_bytes, void* out, void* stream);
+int dbir_gemv(const void* w, int64_t ldw, const void* x, int32_t N, int32_t K, int32_t epilogue, int32_t pack,
+              const float* residual, void* y, int32_t out_kind, void* stream);
+int dbir_argmax(const float* logits, int32_t n, int32_t* token, int32_t* advance, int32_t n_advance, void* stream);
+int dbir_embed_gather(const void* table, int32_t vocab, const int32_t* ids, int32_t n, int32_t dim, float* out,
+                      int64_t ldo, void* stream);
 
 /* ---- small / memory-bound ops ------------------------------------------------------------
  * conv3x3_small_cin : stems with <= 16 input channels; input = virtual concat of two NCHW
