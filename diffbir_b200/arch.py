@@ -525,11 +525,8 @@ def ram_state_dict(ckpt: dict, cfg: dict = None) -> dict:
         if k.endswith("relative_position_bias_table") and v.shape[0] != rows:
             raise ValueError(f"{k}: {v.shape[0]} rows, expected {rows} ((2 * {cfg['window_size']} - 1)^2); "
                              "relative-position tables of other window sizes are not interpolated")
-    for k, shp in ram_shapes(cfg).items():
-        if k not in sd:
-            raise KeyError(f"RAM++ checkpoint is missing {k}")
-        if tuple(sd[k].shape) != tuple(shp):
-            raise ValueError(f"{k}: {tuple(sd[k].shape)} != {shp}")
+    from .engine.common import check_shapes          # imported here: this module needs neither torch nor the library
+    check_shapes(sd, ram_shapes(cfg), "RAM++")
     return sd
 
 

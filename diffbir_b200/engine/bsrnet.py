@@ -21,7 +21,7 @@ from typing import Dict
 import torch
 
 from .. import arch, lib
-from .common import GraphCache, Workspace, f32, pack_conv3x3
+from .common import GraphCache, Workspace, check_shapes, f32, pack_conv3x3, round_up
 
 
 class RRDBNetEngine:
@@ -29,12 +29,7 @@ class RRDBNetEngine:
         self.cfg = dict(arch.RRDBNET_CFG if cfg is None else cfg)
         self.dev = torch.device(device)
         cfg = self.cfg
-        shapes = arch.rrdbnet_shapes(cfg)
-        for k, shp in shapes.items():
-            if k not in sd:
-                raise KeyError(f"RRDBNet checkpoint is missing {k}")
-            if tuple(sd[k].shape) != tuple(shp):
-                raise ValueError(f"{k}: {tuple(sd[k].shape)} != {shp}")
+        check_shapes(sd, arch.rrdbnet_shapes(cfg), "RRDBNet")
         nf, gc = cfg["nf"], cfg["gc"]
         if nf % 64 or (nf + 4 * gc) % 64 or gc % 8:
             raise NotImplementedError("RRDBNetEngine: nf and nf + 4 gc must be multiples of 64, gc of 8")
@@ -51,7 +46,7 @@ class RRDBNetEngine:
                 p = f"RRDB_trunk.{b}.RDB{r}."
                 for k in range(1, 6):
                     cin = nf + (k - 1) * gc
-                    w[p + f"conv{k}.w"] = pack_conv3x3(sd[p + f"conv{k}.weight"], dev, cin_pad=(cin + 63) // 64 * 64)
+                    w[p + f"conv{k}.w"] = pack_conv3x3(sd[p + f"conv{k}.weight"], dev, cin_pad=round_up(cin))
                     w[p + f"conv{k}.b"] = f32(sd[p + f"conv{k}.bias"], dev)
         for nm in ["trunk_conv", "upconv1"] + (["upconv2"] if cfg["sf"] == 4 else []) + ["HRconv"]:
             w[nm + ".w"] = pack_conv3x3(sd[nm + ".weight"], dev)
@@ -83,7 +78,7 @@ class RRDBNetEngine:
                 p = f"RRDB_trunk.{b}.RDB{r}."
                 for k in range(1, 5):                              # x_k = lrelu(conv_k(cat[:, :nf+(k-1)gc]))
                     ck = nf + (k - 1) * gc
-                    ckp = (ck + 63) // 64 * 64
+                    ckp = round_up(ck)
                     lib.gemm(cat, W[p + f"conv{k}.w"], cat[:, ck:], M=M, N=gc, K=9 * ckp, bias=W[p + f"conv{k}.b"],
                              act="lrelu", act_param=0.2, conv=(n, h, wd, ckp, 3), lda=C, ldo=C)
                 out = cur[flip]                                    # x5 * 0.2 + x (bsrnet.py:57-58), fp32

@@ -387,37 +387,42 @@ class CldmEngine:
                    bias=W[l.prefix + "b"], conv=(nb, 2 * h, 2 * w, c, 3),
                    **self._stats_kw(out, nb, l.cout, conv_hw=(2 * h, 2 * w)))
 
-    def _encoder(self, net: _Net, tag: str, x_in, hint, nb, h, w):
-        """Input blocks + middle of ONE net. Returns (list of (tensor, c, h, w) per input block, middle)."""
-        ws, W = self.ws, net.w
+    def _encoder(self, W, tag: str, stems, x_in, h, w):
+        """Input blocks + middle block. stems = ((net, hint), ...), one per problem stacked along the batch: the UNet
+        alone ((U, None)), the ControlNet alone ((Cn, c_img)), or both twins ((U, None), (Cn, c_img)), whose layers
+        past the stems run as grouped launches on W = self.twin_w. Each stem conv writes its problem's rows of the
+        first buffer. Returns (list of (tensor, c, h, w) per input block, middle)."""
+        ws, G, n1 = self.ws, len(stems), x_in.shape[0]
+        nb = G * n1                                         # images of the call, all problems
         outs = []
         cur, ch, cw, cc = None, h, w, 0
-        for bi, blk in enumerate(net.plan.input_blocks):
+        for bi, blk in enumerate(stems[0][0].plan.input_blocks):
             for l in blk.layers:
-                if l.kind == "conv_in":
+                if l.kind == "conv_in":                     # the stems differ (4 vs 4 + 4 input channels)
                     o = ws.get(f"{tag}_hs{bi}", (nb * h * w, l.cout), torch.float32)
-                    c1 = x_in.shape[1]
-                    c2 = hint.shape[1] if hint is not None else 0
-                    lib.conv3x3_small_cin(x_in, hint, c1, c2, nb, h, w, W[l.prefix + "w"],
-                                          W[l.prefix + "b"], l.cout, o)
+                    rows = n1 * h * w
+                    for g, (net, hint) in enumerate(stems):
+                        c2 = hint.shape[1] if hint is not None else 0
+                        lib.conv3x3_small_cin(x_in, hint, x_in.shape[1], c2, n1, h, w, net.w[l.prefix + "w"],
+                                              net.w[l.prefix + "b"], l.cout, o[g * rows:(g + 1) * rows])
                     self._part.pop(o.data_ptr(), None)      # written without GEMM partials
                     cur, cc = o, l.cout
                 elif l.kind == "res":
                     o = ws.get(f"{tag}_hs{bi}", (nb * ch * cw, l.cout), torch.float32)
-                    self._res(W, tag, l, cur, None, cc, 0, nb, ch, cw, o)
+                    self._res(W, tag, l, cur, None, cc, 0, nb, ch, cw, o, G=G)
                     cur, cc = o, l.cout
                 elif l.kind == "attn":
-                    self._attn(W, tag, l, cur, nb, ch, cw)
+                    self._attn(W, tag, l, cur, nb, ch, cw, G=G)
                 elif l.kind == "down":
                     o = ws.get(f"{tag}_hs{bi}", (nb * (ch // 2) * (cw // 2), l.cout), torch.float32)
-                    self._down(W, tag, l, cur, nb, ch, cw, o)
+                    self._down(W, tag, l, cur, nb, ch, cw, o, G=G)
                     cur, cc, ch, cw = o, l.cout, ch // 2, cw // 2
             outs.append((cur, cc, ch, cw))
         mid = ws.get(f"{tag}_mid", (nb * ch * cw, cc), torch.float32)
-        m = net.plan.middle.layers
-        self._res(W, tag, m[0], cur, None, cc, 0, nb, ch, cw, mid)
-        self._attn(W, tag, m[1], mid, nb, ch, cw)
-        self._res(W, tag, m[2], mid, None, cc, 0, nb, ch, cw, mid)
+        m = stems[0][0].plan.middle.layers
+        self._res(W, tag, m[0], cur, None, cc, 0, nb, ch, cw, mid, G=G)
+        self._attn(W, tag, m[1], mid, nb, ch, cw, G=G)
+        self._res(W, tag, m[2], mid, None, cc, 0, nb, ch, cw, mid, G=G)
         return outs, (mid, cc, ch, cw)
 
     def twins_feasible(self, nb: int, h: int, w: int) -> bool:
@@ -437,51 +442,6 @@ class CldmEngine:
             return False
         imgs_per_tile = max(1, 128 // px)              # conv tiles of 128 pixels span this many images
         return nb % imgs_per_tile == 0
-
-    def _encoder_twins(self, x_in, hint, nb, h, w):
-        """UNet encoder + middle and ControlNet as ONE stream of grouped launches: activations are stacked
-        along the batch ([nb UNet images ; nb ControlNet images]), every twin layer is one dbir_gemm with
-        groups = 2 (norm kernels pick the gamma / beta set by image). Halves the launch count of the
-        encoder half of the forward and doubles the wave fill of its single-wave grids.
-        Returns (UNet skips, UNet middle, ControlNet outputs, ControlNet middle) as views of the stacked buffers."""
-        ws, U, Cn, W, tag = self.ws, self.unet, self.cnet, self.twin_w, "g"
-        n2 = 2 * nb
-        outs = []
-        cur, ch, cw, cc = None, h, w, 0
-        for bi, blk in enumerate(U.plan.input_blocks):
-            for l in blk.layers:
-                if l.kind == "conv_in":                     # the stems differ (4 vs 4 + 4 input channels)
-                    o = ws.get(f"g_hs{bi}", (n2 * h * w, l.cout), torch.float32)
-                    half = nb * h * w
-                    lib.conv3x3_small_cin(x_in, None, x_in.shape[1], 0, nb, h, w, U.w[l.prefix + "w"],
-                                          U.w[l.prefix + "b"], l.cout, o[:half])
-                    lib.conv3x3_small_cin(x_in, hint, x_in.shape[1], hint.shape[1], nb, h, w, Cn.w[l.prefix + "w"],
-                                          Cn.w[l.prefix + "b"], l.cout, o[half:])
-                    self._part.pop(o.data_ptr(), None)      # written without GEMM partials
-                    cur, cc = o, l.cout
-                elif l.kind == "res":
-                    o = ws.get(f"g_hs{bi}", (n2 * ch * cw, l.cout), torch.float32)
-                    self._res(W, tag, l, cur, None, cc, 0, n2, ch, cw, o, G=2)
-                    cur, cc = o, l.cout
-                elif l.kind == "attn":
-                    self._attn(W, tag, l, cur, n2, ch, cw, G=2)
-                elif l.kind == "down":
-                    o = ws.get(f"g_hs{bi}", (n2 * (ch // 2) * (cw // 2), l.cout), torch.float32)
-                    self._down(W, tag, l, cur, n2, ch, cw, o, G=2)
-                    cur, cc, ch, cw = o, l.cout, ch // 2, cw // 2
-            outs.append((cur, cc, ch, cw))
-        mid = ws.get("g_mid", (n2 * ch * cw, cc), torch.float32)
-        m = U.plan.middle.layers
-        self._res(W, tag, m[0], cur, None, cc, 0, n2, ch, cw, mid, G=2)
-        self._attn(W, tag, m[1], mid, n2, ch, cw, G=2)
-        self._res(W, tag, m[2], mid, None, cc, 0, n2, ch, cw, mid, G=2)
-
-        def halves(t, c, th, tw):
-            r = nb * th * tw
-            return (t[:r], c, th, tw), (t[r:], c, th, tw)
-        hs, chs = zip(*(halves(*o) for o in outs))
-        umid, cmid = halves(mid, cc, ch, cw)
-        return list(hs), umid, list(chs), cmid
 
     # ------------------------------------------------------------------ CUDA graph of one forward
     def graphed_forward(self, nb: int, c: int, h: int, w: int, control_scales: Sequence[float]):
@@ -524,12 +484,19 @@ class CldmEngine:
         assert nb == self._nb == self.emb_nb, "set_context / set_timesteps batch mismatch"
         ws, U, Cn = self.ws, self.unet, self.cnet
         # 1+2. UNet encoder + middle and the ControlNet. Production shapes: their twin layers run as ONE
-        #      stream of grouped launches on batch-stacked activations (_encoder_twins). Otherwise: UNet
+        #      stream of grouped launches on batch-stacked activations. Otherwise: UNet
         #      on the current stream, ControlNet concurrently on a side stream (fork/join with events so
         #      the pair is also captured as parallel graph branches).
         main = torch.cuda.current_stream()
         if self.twins_feasible(nb, h, w):
-            hs, (mid, mc_, mh, mw), chs, (cmid, cmc, cmh, cmw) = self._encoder_twins(x, c_img, nb, h, w)
+            # activations stacked along the batch ([nb UNet images ; nb ControlNet images]): every twin layer is one
+            # dbir_gemm with groups = 2 (norm kernels pick the gamma / beta set by image), which halves the launch
+            # count of the encoder half and doubles the wave fill of its single-wave grids
+            outs, gmid = self._encoder(self.twin_w, "g", ((U, None), (Cn, c_img)), x, h, w)
+            hs = [(t[:nb * th * tw], c, th, tw) for t, c, th, tw in outs]
+            chs = [(t[nb * th * tw:], c, th, tw) for t, c, th, tw in outs]
+            t, mc_, mh, mw = gmid
+            mid, cmid, (cmc, cmh, cmw) = t[:nb * mh * mw], t[nb * mh * mw:], (mc_, mh, mw)
         elif self.two_streams:
             if self._side is None:
                 self._side = torch.cuda.Stream(device=self.dev)
@@ -537,13 +504,13 @@ class CldmEngine:
             self._ev_fork.record(main)
             self._side.wait_event(self._ev_fork)
             with torch.cuda.stream(self._side):
-                chs, (cmid, cmc, cmh, cmw) = self._encoder(Cn, "c", x, c_img, nb, h, w)
+                chs, (cmid, cmc, cmh, cmw) = self._encoder(Cn.w, "c", ((Cn, c_img),), x, h, w)
                 self._ev_join.record(self._side)
-            hs, (mid, mc_, mh, mw) = self._encoder(U, "u", x, None, nb, h, w)
+            hs, (mid, mc_, mh, mw) = self._encoder(U.w, "u", ((U, None),), x, h, w)
             main.wait_event(self._ev_join)
         else:
-            hs, (mid, mc_, mh, mw) = self._encoder(U, "u", x, None, nb, h, w)
-            chs, (cmid, cmc, cmh, cmw) = self._encoder(Cn, "c", x, c_img, nb, h, w)
+            hs, (mid, mc_, mh, mw) = self._encoder(U.w, "u", ((U, None),), x, h, w)
+            chs, (cmid, cmc, cmh, cmw) = self._encoder(Cn.w, "c", ((Cn, c_img),), x, h, w)
         # zero-convs accumulate scale_i * (W h + b) into the UNet skips / middle in place
         for i, (t, c, th, tw) in enumerate(chs):
             M = nb * th * tw

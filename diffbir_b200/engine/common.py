@@ -1,7 +1,8 @@
-"""Shared engine plumbing: named workspace buffers and weight packing helpers."""
+"""Shared engine plumbing: named workspace buffers, checkpoint checks, weight packing helpers and the pre-norm
+transformer block."""
 from __future__ import annotations
 
-from typing import Dict, Tuple
+from typing import Callable, Dict, Tuple
 
 import torch
 
@@ -79,6 +80,19 @@ class GraphCache:
         return out.clone()
 
 
+def round_up(n: int, m: int = 64) -> int:
+    return (n + m - 1) // m * m
+
+
+def check_shapes(sd: Dict[str, torch.Tensor], shapes, what: str) -> None:
+    """Every key of `shapes` is in the checkpoint `sd` with that shape (other keys are ignored)."""
+    for k, shp in shapes.items():
+        if k not in sd:
+            raise KeyError(f"{what} checkpoint is missing {k}")
+        if tuple(sd[k].shape) != tuple(shp):
+            raise ValueError(f"{k}: {tuple(sd[k].shape)} != {shp}")
+
+
 def op16(t: torch.Tensor, device) -> torch.Tensor:
     return t.to(device=device, dtype=lib.operand_dtype()).contiguous()
 
@@ -103,6 +117,48 @@ def pack_linear(w: torch.Tensor, device, k_pad: int = 0) -> torch.Tensor:
     if k_pad and k_pad > w.shape[1]:
         w = torch.nn.functional.pad(w, (0, k_pad - w.shape[1]))
     return op16(w, device)
+
+
+def pack_gathered(w: torch.Tensor, device, n_pad: int = 0) -> torch.Tensor:
+    """[Cout, Cin, kh, kw] -> op16 [Cout', K] for a GEMM on dbir_patch_gather's patches: k = tap*Cin + c, K zero-padded
+    to a multiple of 64, rows zero-padded to n_pad."""
+    co = w.shape[0]
+    flat = w.permute(0, 2, 3, 1).reshape(co, -1)
+    return op16(torch.nn.functional.pad(flat, (0, round_up(flat.shape[1]) - flat.shape[1], 0, max(0, n_pad - co))),
+                device)
+
+
+def pack_swin_block(w: Dict[str, torch.Tensor], dst: str, sd: Dict[str, torch.Tensor], src: str, device,
+                    k_pad: int = 0, hid_pad: int = 0) -> None:
+    """Swin block `src` of a checkpoint (norm1, attn.qkv, attn.proj, attn.relative_position_bias_table, norm2,
+    mlp.fc1, mlp.fc2) -> w[dst + prenorm_block's names] and w[dst + "rpb"]. GEMM K is zero-padded to k_pad, fc2's to
+    hid_pad."""
+    for i in (1, 2):
+        w[f"{dst}ln{i}.w"] = f32(sd[f"{src}norm{i}.weight"], device)
+        w[f"{dst}ln{i}.b"] = f32(sd[f"{src}norm{i}.bias"], device)
+    for nm, key, kp in (("qkv", "attn.qkv", k_pad), ("proj", "attn.proj", k_pad), ("fc1", "mlp.fc1", k_pad),
+                        ("fc2", "mlp.fc2", hid_pad)):
+        w[dst + nm + ".w"] = pack_linear(sd[src + key + ".weight"], device, kp)
+        w[dst + nm + ".b"] = f32(sd[src + key + ".bias"], device)
+    w[dst + "rpb"] = f32(sd[src + "attn.relative_position_bias_table"], device)
+
+
+def prenorm_block(W: Dict[str, torch.Tensor], p: str, t: torch.Tensor, bufs, M: int, c: int, hidden: int, lds,
+                  act: str, eps: float, attend: Callable[[torch.Tensor, torch.Tensor], None]) -> None:
+    """One pre-norm transformer block in place on the fp32 token stream t [M, c] (row stride lds[0]):
+    t += proj(attention(qkv(LN1(t)))), then t += fc2(act(fc1(LN2(t)))).
+    bufs = (ln16, qkv16, att16, hid16): op16 work buffers. lds = row strides of (t / ln16 / att16, qkv16, hid16);
+    each is also the K of the GEMM that reads that buffer (weights zero-padded to it). attend(qkv16, att16) enqueues
+    the attention. Weights: W[p + "ln1.w" / "ln1.b" / "qkv.w" / "qkv.b" / "proj.*" / "ln2.*" / "fc1.*" / "fc2.*"]."""
+    ln16, qkv, att, hid = bufs
+    ldt, ldqkv, ldh = lds
+    lib.layernorm(t, ldt, M, c, W[p + "ln1.w"], W[p + "ln1.b"], ln16, ldt, eps=eps)
+    lib.gemm(ln16, W[p + "qkv.w"], qkv, M=M, N=3 * c, K=ldt, bias=W[p + "qkv.b"], ldo=ldqkv)
+    attend(qkv, att)
+    lib.gemm(att, W[p + "proj.w"], t, M=M, N=c, K=ldt, bias=W[p + "proj.b"], residual=t, ldo=ldt, ldr=ldt)
+    lib.layernorm(t, ldt, M, c, W[p + "ln2.w"], W[p + "ln2.b"], ln16, ldt, eps=eps)
+    lib.gemm(ln16, W[p + "fc1.w"], hid, M=M, N=hidden, K=ldt, bias=W[p + "fc1.b"], act=act, ldo=ldh)
+    lib.gemm(hid, W[p + "fc2.w"], t, M=M, N=c, K=ldh, bias=W[p + "fc2.b"], residual=t, ldo=ldt, ldr=ldt)
 
 
 def geglu_tile(c: int) -> int:

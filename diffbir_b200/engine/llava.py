@@ -26,6 +26,7 @@ from typing import Dict, List, Optional, Sequence
 import torch
 
 from .. import arch, lib
+from .common import f32, op16, prenorm_block, round_up
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)     # CLIPImageProcessor image_mean / image_std
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -65,28 +66,20 @@ class LlavaEngine:
         assert vw == cfg["v_heads"] * VISION_HEAD_DIM and d == H * arch.LLAVA_HEAD_DIM
         self.bn = swiglu_tile(f)
 
-        def take(k):
-            return sd.pop(k)
-
-        def o16(t):
-            return t.to(device=dev, dtype=dt).contiguous()
-
-        def f32(t):
-            return t.to(device=dev, dtype=torch.float32).contiguous()
-
+        take = sd.pop
         w = {}
         v = arch.VISION_PREFIX + "vision_model."
         r = cfg["patch"]
         self.stem_c = 3 * r * r
-        self.stem_cp = -(-self.stem_c // 64) * 64                      # 588 -> 640
+        self.stem_cp = round_up(self.stem_c)                           # 588 -> 640
         pe = take(v + "embeddings.patch_embedding.weight").to(dev, torch.float32)
         pe = pe / torch.tensor(CLIP_STD, device=dev).view(1, 3, 1, 1)
-        w["pe"] = o16(torch.nn.functional.pad(pe.reshape(vw, self.stem_c), (0, self.stem_cp - self.stem_c)))
-        pos = f32(take(v + "embeddings.position_embedding.weight"))
+        w["pe"] = op16(torch.nn.functional.pad(pe.reshape(vw, self.stem_c), (0, self.stem_cp - self.stem_c)), dev)
+        pos = f32(take(v + "embeddings.position_embedding.weight"), dev)
         self.vemb = torch.empty(self.patches + 1, vw, device=dev)
-        self.vemb[0] = f32(take(v + "embeddings.class_embedding")) + pos[0]      # constant class-token row
+        self.vemb[0] = f32(take(v + "embeddings.class_embedding"), dev) + pos[0]      # constant class-token row
         w["pos"] = pos[1:].contiguous()
-        w["pre.w"], w["pre.b"] = f32(take(v + "pre_layrnorm.weight")), f32(take(v + "pre_layrnorm.bias"))
+        w["pre.w"], w["pre.b"] = f32(take(v + "pre_layrnorm.weight"), dev), f32(take(v + "pre_layrnorm.bias"), dev)
         for i in range(cfg["v_layers"]):
             p = f"{v}encoder.layers.{i}."
             keys = [k for k in sd if k.startswith(p)]
@@ -94,33 +87,35 @@ class LlavaEngine:
                 for k in keys:
                     del sd[k]
                 continue
-            o = f"v{i}."
-            w[o + "qkv.w"] = o16(torch.cat([take(p + f"self_attn.{n}_proj.weight").to(dev) for n in "qkv"]))
-            w[o + "qkv.b"] = f32(torch.cat([take(p + f"self_attn.{n}_proj.bias").to(dev) for n in "qkv"]))
-            for src, dst in (("self_attn.out_proj", "out"), ("mlp.fc1", "fc1"), ("mlp.fc2", "fc2")):
-                w[o + dst + ".w"], w[o + dst + ".b"] = o16(take(p + src + ".weight")), f32(take(p + src + ".bias"))
-            for nm in ("layer_norm1", "layer_norm2"):
-                w[o + nm + ".w"], w[o + nm + ".b"] = f32(take(p + nm + ".weight")), f32(take(p + nm + ".bias"))
+            o = f"v{i}."                                                # prenorm_block's names
+            w[o + "qkv.w"] = op16(torch.cat([take(p + f"self_attn.{n}_proj.weight").to(dev) for n in "qkv"]), dev)
+            w[o + "qkv.b"] = f32(torch.cat([take(p + f"self_attn.{n}_proj.bias").to(dev) for n in "qkv"]), dev)
+            for src, dst in (("self_attn.out_proj", "proj"), ("mlp.fc1", "fc1"), ("mlp.fc2", "fc2")):
+                w[o + dst + ".w"] = op16(take(p + src + ".weight"), dev)
+                w[o + dst + ".b"] = f32(take(p + src + ".bias"), dev)
+            for src, dst in (("layer_norm1", "ln1"), ("layer_norm2", "ln2")):
+                w[o + dst + ".w"] = f32(take(p + src + ".weight"), dev)
+                w[o + dst + ".b"] = f32(take(p + src + ".bias"), dev)
         for k in [k for k in sd if k.startswith(v + "post_layernorm")]:
             del sd[k]
         for i in (0, 2):
-            w[f"mm{i}.w"] = o16(take(f"model.mm_projector.{i}.weight"))
-            w[f"mm{i}.b"] = f32(take(f"model.mm_projector.{i}.bias"))
-        w["embed"] = o16(take("model.embed_tokens.weight"))
+            w[f"mm{i}.w"] = op16(take(f"model.mm_projector.{i}.weight"), dev)
+            w[f"mm{i}.b"] = f32(take(f"model.mm_projector.{i}.bias"), dev)
+        w["embed"] = op16(take("model.embed_tokens.weight"), dev)
         hb = self.bn // 2
         for i in range(cfg["layers"]):
             p, o = f"model.layers.{i}.", f"l{i}."
-            w[o + "qkv"] = o16(torch.cat([take(p + f"self_attn.{n}_proj.weight").to(dev, dt) for n in "qkv"]))
-            w[o + "o"] = o16(take(p + "self_attn.o_proj.weight"))
+            w[o + "qkv"] = op16(torch.cat([take(p + f"self_attn.{n}_proj.weight").to(dev, dt) for n in "qkv"]), dev)
+            w[o + "o"] = op16(take(p + "self_attn.o_proj.weight"), dev)
             up = take(p + "mlp.up_proj.weight").to(dev, dt).view(f // hb, hb, d)       # values
             gate = take(p + "mlp.gate_proj.weight").to(dev, dt).view(f // hb, hb, d)   # gates
             w[o + "gu"] = torch.cat([up, gate], dim=1).reshape(2 * f, d).contiguous()
             del up, gate
-            w[o + "down"] = o16(take(p + "mlp.down_proj.weight"))
-            w[o + "ln1"] = f32(take(p + "input_layernorm.weight"))
-            w[o + "ln2"] = f32(take(p + "post_attention_layernorm.weight"))
-        w["norm"] = f32(take("model.norm.weight"))
-        w["lm_head"] = o16(take("lm_head.weight"))
+            w[o + "down"] = op16(take(p + "mlp.down_proj.weight"), dev)
+            w[o + "ln1"] = f32(take(p + "input_layernorm.weight"), dev)
+            w[o + "ln2"] = f32(take(p + "post_attention_layernorm.weight"), dev)
+        w["norm"] = f32(take("model.norm.weight"), dev)
+        w["lm_head"] = op16(take("lm_head.weight"), dev)
         assert not sd, f"unused weights: {sorted(sd)[:4]}"
         self.w = w
 
@@ -228,20 +223,14 @@ class LlavaEngine:
         lib.gemm(self.stem16, W["pe"], self.vemb[1:], M=P, N=vw, K=self.stem_cp, residual=W["pos"])
         t = self.t
         lib.layernorm(self.vemb, vw, nv, vw, W["pre.w"], W["pre.b"], t, vw, eps=cfg["v_eps"])
-        heads, ld = cfg["v_heads"], 3 * vw
+        heads, ld, vi = cfg["v_heads"], 3 * vw, cfg["v_intermediate"]
+
+        def attend(q, att):
+            lib.attention(q, q[:, vw:], q[:, 2 * vw:], att, batch=1, heads=heads, sq=nv, skv=nv, ldq=ld, ldk=ld, ldv=ld,
+                          ldo=vw, ws=self.vattn_ws)
+        bufs = (self.ln16, self.vqkv16, self.vatt16, self.vhid16)
         for i in range(self.v_run):
-            o = f"v{i}."
-            lib.layernorm(t, vw, nv, vw, W[o + "layer_norm1.w"], W[o + "layer_norm1.b"], self.ln16, vw, eps=cfg["v_eps"])
-            lib.gemm(self.ln16, W[o + "qkv.w"], self.vqkv16, M=nv, N=3 * vw, K=vw, bias=W[o + "qkv.b"])
-            q = self.vqkv16
-            lib.attention(q, q[:, vw:], q[:, 2 * vw:], self.vatt16, batch=1, heads=heads, sq=nv, skv=nv, ldq=ld,
-                          ldk=ld, ldv=ld, ldo=vw, ws=self.vattn_ws)
-            lib.gemm(self.vatt16, W[o + "out.w"], t, M=nv, N=vw, K=vw, bias=W[o + "out.b"], residual=t)
-            lib.layernorm(t, vw, nv, vw, W[o + "layer_norm2.w"], W[o + "layer_norm2.b"], self.ln16, vw, eps=cfg["v_eps"])
-            lib.gemm(self.ln16, W[o + "fc1.w"], self.vhid16, M=nv, N=cfg["v_intermediate"], K=vw, bias=W[o + "fc1.b"],
-                     act="quick_gelu")
-            lib.gemm(self.vhid16, W[o + "fc2.w"], t, M=nv, N=vw, K=cfg["v_intermediate"], bias=W[o + "fc2.b"],
-                     residual=t)
+            prenorm_block(W, f"v{i}.", t, bufs, nv, vw, vi, (vw, ld, vi), "quick_gelu", cfg["v_eps"], attend)
         lib.axpby_cast(t[1:], 1.0, None, P, vw, y16=self.feat16, ld16=vw)          # select_feature "patch"
 
     def _project(self, out: torch.Tensor):

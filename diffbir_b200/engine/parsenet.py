@@ -20,17 +20,10 @@ import numpy as np
 import torch
 
 from .. import arch, lib
-from .common import Workspace, f32, pack_linear
+from .common import Workspace, f32, pack_gathered, round_up
 
 SIZE = 512
 MAX_BATCH = 4            # faces per forward
-
-
-def _pack(wt: torch.Tensor, dev, n_pad: int = 0) -> torch.Tensor:
-    co = wt.shape[0]
-    flat = wt.permute(0, 2, 3, 1).reshape(co, -1)
-    flat = torch.nn.functional.pad(flat, (0, (-flat.shape[1]) % 64, 0, max(0, n_pad - co)))
-    return pack_linear(flat, dev)
 
 
 class ParseNetEngine:
@@ -46,7 +39,7 @@ class ParseNetEngine:
             wt, b = sd[name + "conv2d.weight"], sd.get(name + "conv2d.bias")
             if bn:
                 wt, b = arch.fold_bn(wt, sd, name + "norm.norm", b)
-            w[name + "w"] = _pack(wt, dev, n_pad)
+            w[name + "w"] = pack_gathered(wt, dev, n_pad)
             w[name + "b"] = f32(torch.nn.functional.pad(b.float(), (0, max(0, n_pad - b.shape[0]))), dev)
 
         layer("encoder.0.")
@@ -56,14 +49,14 @@ class ParseNetEngine:
             layer(p + "conv1.", bn=True)
             layer(p + "conv2.", bn=True)
         self.classes = self.cfg["parsing_ch"]
-        self.n_mask = (self.classes + 31) // 32 * 32          # 19 logits in rows of 32 (16-byte GEMM output rows)
+        self.n_mask = round_up(self.classes, 32)               # 19 logits in rows of 32 (16-byte GEMM output rows)
         layer("out_mask_conv.", n_pad=self.n_mask)
         self.w = w
 
     def _conv(self, x, n, h, w, c, name, out, *, stride=1, up2=False, act=False, residual=None, g=None):
         """ConvLayer: reflection-padded 3x3 conv of op16 x [n*h*w, c]; returns (ho, wo, gathered patches)."""
         ho, wo = lib.patch_gather_shape(h, w, 3, stride, up2)
-        kp = (9 * c + 63) // 64 * 64
+        kp = round_up(9 * c)
         if g is None:
             g = self.ws.get("g", (n * ho * wo, kp), lib.operand_dtype())
             lib.patch_gather(x, c, n, h, w, c, 3, stride, kp, g, reflect=True, up2=up2)

@@ -24,7 +24,7 @@ from typing import Dict
 import torch
 
 from .. import arch, lib
-from .common import GraphCache, Workspace, f32, op16, pack_linear
+from .common import GraphCache, Workspace, f32, op16, pack_linear, pack_swin_block, prenorm_block, round_up
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)      # ram/transform.py
 IMAGENET_STD = (0.229, 0.224, 0.225)
@@ -51,7 +51,7 @@ class RamPlusEngine:
         pe = sd[p + "patch_embed.proj.weight"].float()
         c0, r = pe.shape[0], cfg["patch_size"]
         self.stem_c = 3 * r * r
-        self.stem_cp = -(-self.stem_c // 64) * 64                       # 48 -> 64
+        self.stem_cp = round_up(self.stem_c)                            # 48 -> 64
         std = torch.tensor(IMAGENET_STD).view(1, 3, 1, 1)
         w["pe.w"] = pack_linear((pe / std).reshape(c0, self.stem_c), dev, self.stem_cp)   # (c, dy, dx) = unshuffle order
         w["pe.b"] = f32(sd[p + "patch_embed.proj.bias"], dev)
@@ -59,19 +59,7 @@ class RamPlusEngine:
         w["pe.norm.b"] = f32(sd[p + "patch_embed.norm.bias"], dev)
         for i, (c, _, _, _, shifts) in enumerate(self.stages):
             for b in range(len(shifts)):
-                q, o = f"{p}layers.{i}.blocks.{b}.", f"{i}.{b}."
-                for nm in ("norm1", "norm2"):
-                    w[o + nm + ".w"] = f32(sd[q + nm + ".weight"], dev)
-                    w[o + nm + ".b"] = f32(sd[q + nm + ".bias"], dev)
-                w[o + "qkv.w"] = pack_linear(sd[q + "attn.qkv.weight"], dev)
-                w[o + "qkv.b"] = f32(sd[q + "attn.qkv.bias"], dev)
-                w[o + "proj.w"] = pack_linear(sd[q + "attn.proj.weight"], dev)
-                w[o + "proj.b"] = f32(sd[q + "attn.proj.bias"], dev)
-                w[o + "rpb"] = f32(sd[q + "attn.relative_position_bias_table"], dev)
-                w[o + "fc1.w"] = pack_linear(sd[q + "mlp.fc1.weight"], dev)
-                w[o + "fc1.b"] = f32(sd[q + "mlp.fc1.bias"], dev)
-                w[o + "fc2.w"] = pack_linear(sd[q + "mlp.fc2.weight"], dev)
-                w[o + "fc2.b"] = f32(sd[q + "mlp.fc2.bias"], dev)
+                pack_swin_block(w, f"{i}.{b}.", sd, f"{p}layers.{i}.blocks.{b}.", dev)
             if i < len(self.stages) - 1:
                 q = f"{p}layers.{i}.downsample."
                 w[f"{i}.merge.w"] = f32(sd[q + "norm.weight"], dev)
@@ -158,20 +146,14 @@ class RamPlusEngine:
         lib.layernorm(pe, c0, M, c0, W["pe.norm.w"], W["pe.norm.b"], t, c0)
         for i, (c, side, heads, win, shifts) in enumerate(self.stages):
             M = nb * side * side
-            ln16 = ws.get("ln16", (M, c), dt)
-            qkv = ws.get("qkv16", (M, 3 * c), dt)
-            att = ws.get("att16", (M, c), dt)
-            hid = ws.get("hid16", (M, cfg["mlp_ratio"] * c), dt)
+            hidden = cfg["mlp_ratio"] * c
+            bufs = (ws.get("ln16", (M, c), dt), ws.get("qkv16", (M, 3 * c), dt), ws.get("att16", (M, c), dt),
+                    ws.get("hid16", (M, hidden), dt))
             for b, shift in enumerate(shifts):
                 o = f"{i}.{b}."
-                lib.layernorm(t, c, M, c, W[o + "norm1.w"], W[o + "norm1.b"], ln16, c)
-                lib.gemm(ln16, W[o + "qkv.w"], qkv, M=M, N=3 * c, K=c, bias=W[o + "qkv.b"])
-                lib.window_attention(qkv, 3 * c, nb, side, side, heads, HEAD_DIM, shift, W[o + "rpb"], -100.0, att, c,
-                                     window=win)
-                lib.gemm(att, W[o + "proj.w"], t, M=M, N=c, K=c, bias=W[o + "proj.b"], residual=t)
-                lib.layernorm(t, c, M, c, W[o + "norm2.w"], W[o + "norm2.b"], ln16, c)
-                lib.gemm(ln16, W[o + "fc1.w"], hid, M=M, N=cfg["mlp_ratio"] * c, K=c, bias=W[o + "fc1.b"], act="gelu")
-                lib.gemm(hid, W[o + "fc2.w"], t, M=M, N=c, K=cfg["mlp_ratio"] * c, bias=W[o + "fc2.b"], residual=t)
+                prenorm_block(W, o, t, bufs, M, c, hidden, (c, 3 * c, hidden), "gelu", 1e-5,
+                              lambda qkv, att: lib.window_attention(qkv, 3 * c, nb, side, side, heads, HEAD_DIM, shift,
+                                                                    W[o + "rpb"], -100.0, att, c, window=win))
             if i < len(self.stages) - 1:
                 m16 = ws.get("merge16", (M // 4, 4 * c), dt)
                 lib.swin_patch_merge(t, c, nb, side, side, c, W[f"{i}.merge.w"], W[f"{i}.merge.b"], m16, 4 * c)

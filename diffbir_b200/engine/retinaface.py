@@ -24,13 +24,9 @@ import numpy as np
 import torch
 
 from .. import arch, lib
-from .common import Workspace, f32, op16, pack_conv3x3, pack_linear
+from .common import Workspace, f32, pack_conv3x3, pack_gathered, pack_linear, round_up
 
 DETECTOR_MEAN = (104.0, 117.0, 123.0)
-
-
-def _pad64(k: int) -> int:
-    return (k + 63) // 64 * 64
 
 
 class RetinaFaceEngine:
@@ -47,10 +43,8 @@ class RetinaFaceEngine:
                 w[name + ".w"] = pack_linear(wf, dev)
             elif mode == "3x3":
                 w[name + ".w"] = pack_conv3x3(wf, dev)
-            else:                                              # gathered patches: K = taps * C, zero-padded to 64
-                co = wf.shape[0]
-                flat = wf.permute(0, 2, 3, 1).reshape(co, -1)
-                w[name + ".w"] = pack_linear(flat, dev, _pad64(flat.shape[1]))
+            else:
+                w[name + ".w"] = pack_gathered(wf, dev)
             w[name + ".b"] = f32(bf, dev)
 
         conv("stem", sd["body.conv1.weight"], "body.bn1", "gather")
@@ -85,7 +79,7 @@ class RetinaFaceEngine:
 
     def _gathered(self, x, c, h, w, ksize, stride, name, out, tag, act=True):
         ho, wo = lib.patch_gather_shape(h, w, ksize, stride)
-        kp = _pad64(ksize * ksize * c)
+        kp = round_up(ksize * ksize * c)
         g = self.ws.get(tag, (ho * wo, kp), lib.operand_dtype())
         lib.patch_gather(x, c, 1, h, w, c, ksize, stride, kp, g)
         self._gemm(g, name, out, ho * wo, kp, act=act)

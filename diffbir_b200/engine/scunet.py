@@ -19,7 +19,7 @@ from typing import Dict
 import torch
 
 from .. import arch, lib
-from .common import GraphCache, Workspace, f32, pack_conv3x3, pack_linear
+from .common import GraphCache, Workspace, check_shapes, f32, pack_conv3x3, pack_linear
 
 HEAD_DIM = 32
 
@@ -30,12 +30,7 @@ class SCUNetEngine:
         self.cfg["config"] = tuple(self.cfg["config"])
         self.dev = torch.device(device)
         cfg = self.cfg
-        shapes = arch.scunet_shapes(cfg)
-        for k, shp in shapes.items():
-            if k not in sd:
-                raise KeyError(f"SCUNet checkpoint is missing {k}")
-            if tuple(sd[k].shape) != tuple(shp):
-                raise ValueError(f"{k}: {tuple(sd[k].shape)} != {shp}")
+        check_shapes(sd, arch.scunet_shapes(cfg), "SCUNet")
         if cfg["dim"] % 64:
             raise NotImplementedError("SCUNetEngine: dim must be a multiple of 64")
         self.ws = Workspace(self.dev)

@@ -16,11 +16,8 @@ from typing import Dict
 import torch
 
 from .. import arch, lib
-from .common import GraphCache, Workspace, f32, op16, pack_conv3x3, pack_linear
-
-
-def _pad_to(n: int, m: int) -> int:
-    return (n + m - 1) // m * m
+from .common import (GraphCache, Workspace, check_shapes, f32, pack_conv3x3, pack_swin_block, prenorm_block,
+                     round_up)
 
 
 class SwinIREngine:
@@ -32,24 +29,19 @@ class SwinIREngine:
             sd = sd["state_dict"]
         if next(iter(sd)).startswith("module."):
             sd = {k[len("module."):]: v for k, v in sd.items()}
-        shapes = arch.swinir_shapes(cfg)
-        for k, shp in shapes.items():
-            if k not in sd:
-                raise KeyError(f"SwinIR checkpoint is missing {k}")
-            if tuple(sd[k].shape) != tuple(shp):
-                raise ValueError(f"{k}: {tuple(sd[k].shape)} != {shp}")
+        check_shapes(sd, arch.swinir_shapes(cfg), "SwinIR")
         assert cfg["window_size"] == 8 and set(cfg["num_heads"]) == {6} and cfg["embed_dim"] == 180, \
             "window attention kernel is built for window 8, 6 heads x 30"
         self.ws = Workspace(self.dev)
         self.graphs = GraphCache(self.ws)       # ~360 launches per image replayed as one graph per input shape
         self.op_dtype = lib.operand_dtype()
         c = cfg["embed_dim"]
-        self.c, self.cp = c, _pad_to(c, 64)                     # 180 -> 192
+        self.c, self.cp = c, round_up(c)                        # 180 -> 192
         self.hid = int(c * cfg["mlp_ratio"])
-        self.hidp = _pad_to(self.hid, 64)                       # 360 -> 384
-        self.qkv_ld = _pad_to(3 * c, 8)                         # 540 -> 544
+        self.hidp = round_up(self.hid)                          # 360 -> 384
+        self.qkv_ld = round_up(3 * c, 8)                        # 540 -> 544
         self.in_ch = cfg["in_chans"] * cfg["unshuffle_scale"] ** 2   # 192
-        self.in_chp = _pad_to(self.in_ch, 64)
+        self.in_chp = round_up(self.in_ch)
         self.nf = cfg.get("num_feat", 64)
         dev, w = self.dev, {}
         self.w = w
@@ -61,18 +53,7 @@ class SwinIREngine:
         for li, depth in enumerate(cfg["depths"]):
             for bi in range(depth):
                 p = f"layers.{li}.residual_group.blocks.{bi}."
-                for nm in ("norm1", "norm2"):
-                    w[p + nm + ".weight"] = f32(sd[p + nm + ".weight"], dev)
-                    w[p + nm + ".bias"] = f32(sd[p + nm + ".bias"], dev)
-                w[p + "qkv.w"] = pack_linear(sd[p + "attn.qkv.weight"], dev, self.cp)
-                w[p + "qkv.b"] = f32(sd[p + "attn.qkv.bias"], dev)
-                w[p + "proj.w"] = pack_linear(sd[p + "attn.proj.weight"], dev, self.cp)
-                w[p + "proj.b"] = f32(sd[p + "attn.proj.bias"], dev)
-                w[p + "rpb"] = f32(sd[p + "attn.relative_position_bias_table"], dev)
-                w[p + "fc1.w"] = pack_linear(sd[p + "mlp.fc1.weight"], dev, self.cp)
-                w[p + "fc1.b"] = f32(sd[p + "mlp.fc1.bias"], dev)
-                w[p + "fc2.w"] = pack_linear(sd[p + "mlp.fc2.weight"], dev, self.hidp)
-                w[p + "fc2.b"] = f32(sd[p + "mlp.fc2.bias"], dev)
+                pack_swin_block(w, p, sd, p, dev, self.cp, self.hidp)
             w[f"layers.{li}.conv.w"] = pack_conv3x3(sd[f"layers.{li}.conv.weight"], dev, self.cp)
             w[f"layers.{li}.conv.b"] = f32(sd[f"layers.{li}.conv.bias"], dev)
         w["conv_after_body.w"] = pack_conv3x3(sd["conv_after_body.weight"], dev, self.cp)
@@ -117,9 +98,8 @@ class SwinIREngine:
         t = ws.get("tok", (M, cp), torch.float32, zero=True)
         ln16 = ws.get("ln16", (M, cp), dt)
         lib.layernorm(feat0, cp, M, c, W["patch_embed.norm.weight"], W["patch_embed.norm.bias"], t, cp)
-        qkv = ws.get("qkv16", (M, self.qkv_ld), dt, zero=True)
-        att = ws.get("att16", (M, cp), dt, zero=True)
-        hid = ws.get("hid16", (M, self.hidp), dt, zero=True)
+        bufs = (ln16, ws.get("qkv16", (M, self.qkv_ld), dt, zero=True), ws.get("att16", (M, cp), dt, zero=True),
+                ws.get("hid16", (M, self.hidp), dt, zero=True))
         rstb_in = ws.get("rstb_in", (M, cp), torch.float32, zero=True)
         img16 = ws.get("img16", (M, cp), dt)
         for li, depth in enumerate(cfg["depths"]):
@@ -127,16 +107,9 @@ class SwinIREngine:
             for bi in range(depth):
                 p = f"layers.{li}.residual_group.blocks.{bi}."
                 shift = 0 if bi % 2 == 0 else 4
-                lib.layernorm(t, cp, M, c, W[p + "norm1.weight"], W[p + "norm1.bias"], ln16, cp)
-                lib.gemm(ln16, W[p + "qkv.w"], qkv, M=M, N=3 * c, K=cp, bias=W[p + "qkv.b"], ldo=self.qkv_ld)
-                lib.window_attention(qkv, self.qkv_ld, nb, h, w, 6, 30, shift, W[p + "rpb"], -100.0, att, cp)
-                lib.gemm(att, W[p + "proj.w"], t, M=M, N=c, K=cp, bias=W[p + "proj.b"], residual=t,
-                         ldo=cp, ldr=cp)
-                lib.layernorm(t, cp, M, c, W[p + "norm2.weight"], W[p + "norm2.bias"], ln16, cp)
-                lib.gemm(ln16, W[p + "fc1.w"], hid, M=M, N=self.hid, K=cp, bias=W[p + "fc1.b"], act="gelu",
-                         ldo=self.hidp)
-                lib.gemm(hid, W[p + "fc2.w"], t, M=M, N=c, K=self.hidp, bias=W[p + "fc2.b"], residual=t,
-                         ldo=cp, ldr=cp)
+                prenorm_block(W, p, t, bufs, M, c, self.hid, (cp, self.qkv_ld, self.hidp), "gelu", 1e-5,
+                              lambda qkv, att: lib.window_attention(qkv, self.qkv_ld, nb, h, w, 6, 30, shift,
+                                                                    W[p + "rpb"], -100.0, att, cp))
             # RSTB tail: conv3x3 over the token image + residual (swinir.py:487-488)
             lib.gn_apply(t, None, cp, 0, nb, h, w, None, None, None, img16, norm=False, silu=False)
             lib.gemm(img16, W[f"layers.{li}.conv.w"], t, M=M, N=c, K=9 * cp, bias=W[f"layers.{li}.conv.b"],

@@ -22,7 +22,7 @@ from typing import Dict
 import torch
 
 from .. import arch, lib
-from .common import GraphCache, Workspace, f32, op16, pack_conv3x3, pack_linear
+from .common import GraphCache, Workspace, check_shapes, f32, op16, pack_conv3x3, pack_linear
 
 
 class VaeEngine:
@@ -30,11 +30,7 @@ class VaeEngine:
         self.cfg = dict(arch.VAE_CFG if cfg is None else cfg)
         self.dev = torch.device(device)
         shapes = arch.vae_shapes(self.cfg)
-        for k, shp in shapes.items():
-            if k not in sd:
-                raise KeyError(f"VAE checkpoint is missing {k}")
-            if tuple(sd[k].shape) != tuple(shp):
-                raise ValueError(f"{k}: {tuple(sd[k].shape)} != {shp}")
+        check_shapes(sd, shapes, "VAE")
         self.ws = Workspace(self.dev)
         self.graphs = GraphCache(self.ws)       # decode / encode replayed as one graph per input shape
         self.op_dtype = lib.operand_dtype()

@@ -14,6 +14,8 @@ from typing import Dict, List, Optional
 import torch
 import torch.nn.functional as F
 
+from ..engine.common import GraphCache
+
 
 class TextTower:
     def __init__(self, sd: Dict[str, torch.Tensor], heads: int = 16, layer: str = "penultimate",
@@ -24,31 +26,16 @@ class TextTower:
         self.skip_last = 1 if layer == "penultimate" else 0
         self.n_layers = 1 + max(int(k.split(".")[2]) for k in sd if k.startswith("transformer.resblocks."))
         self.context_length = sd["positional_embedding"].shape[0]
-        self._graphs = {}            # token shape -> (CUDAGraph, static tokens, static output)
-        self.use_graphs = True
+        self.graphs = GraphCache() if self.dev.type == "cuda" else None
 
     @torch.no_grad()
     def __call__(self, tokens: torch.Tensor) -> torch.Tensor:
         """tokens int64 [B, 77] -> fp32 [B, 77, width] (model/clip.py:37-59). On CUDA the ~280 small
         library kernels of the tower are replayed as one CUDA graph per batch shape."""
         tokens = tokens.to(self.dev)
-        if not (self.use_graphs and self.dev.type == "cuda") or torch.cuda.is_current_stream_capturing():
+        if self.graphs is None:
             return self._forward(tokens)
-        key = tuple(tokens.shape)
-        hit = self._graphs.get(key)
-        if hit is None:
-            st = tokens.clone()
-            self._forward(st)                                   # warm-up (cuBLAS workspaces, SDPA selection)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                out = self._forward(st)
-            hit = (g, st, out)
-            self._graphs[key] = hit
-        g, st, out = hit
-        st.copy_(tokens)
-        g.replay()
-        return out.clone()
+        return self.graphs.run(tuple(tokens.shape), self._forward, tokens)
 
     def _forward(self, tokens: torch.Tensor) -> torch.Tensor:
         sd = self.sd
