@@ -5,6 +5,7 @@ YAML's `train:` block holds (`sd_path`, `swinir_path`) plus `--ckpt`; stage 1 is
 of the LQ image. The YAML is read with PyYAML (the reference's training configs use no OmegaConf interpolation).
 `--synthetic` only swaps the BPE vocabulary file for the hash tokenizer (random-weight checkpoints in the tests)."""
 from argparse import Namespace
+from typing import Optional
 
 import numpy as np
 import yaml
@@ -13,11 +14,13 @@ from PIL import Image
 from ..pipeline import SwinIRPipeline
 from ..utils.common import instantiate_from_config
 from .loop import InferenceLoop, check_supported, load_checkpoint
+from .ranks import Ranks
 
 
 class CustomInferenceLoop(InferenceLoop):
-    def __init__(self, args: Namespace) -> None:
+    def __init__(self, args: Namespace, ranks: Optional[Ranks] = None) -> None:
         self.args = args
+        self.ranks = ranks
         check_supported(args)
         if not args.train_cfg or not args.ckpt:
             raise ValueError("--version custom needs --train_cfg (the stage-2 training YAML) and --ckpt (ControlNet weights)")

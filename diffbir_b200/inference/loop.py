@@ -9,7 +9,7 @@ import csv
 import os
 from argparse import Namespace
 from pathlib import Path
-from typing import Generator, List
+from typing import Generator, List, Optional
 
 import numpy as np
 import torch
@@ -19,6 +19,7 @@ from PIL import Image
 from ..utils.caption import Captioner, EmptyCaptioner
 from ..utils.common import instantiate_from_config
 from .pretrained_models import default_weights_dir, resolve
+from .ranks import Ranks
 
 CONFIG_DIR = Path(__file__).resolve().parents[2] / "configs" / "inference"
 SUPPORTED_SAMPLERS = ("dpm++_m2", "spaced", "ddim", "edm_euler", "edm_euler_a", "edm_heun", "edm_dpm_2", "edm_dpm_2_a", "edm_lms",
@@ -109,9 +110,11 @@ def prompt_with_caption(caption: str, pos_prompt: str) -> str:
 
 class InferenceLoop:
     captioner: Captioner = EmptyCaptioner("cuda")      # replaced by load_captioner
+    ranks: Optional[Ranks] = None                       # set under torchrun (inference/ranks.py)
 
-    def __init__(self, args: Namespace) -> None:
+    def __init__(self, args: Namespace, ranks: Optional[Ranks] = None) -> None:
         self.args = args
+        self.ranks = ranks
         check_supported(args)
         self.loop_ctx = {}
         self.pipeline = None
@@ -130,10 +133,16 @@ class InferenceLoop:
     def load_pipeline(self) -> None:
         raise NotImplementedError
 
+    def pipelines(self) -> list:
+        """Every pipeline the loop runs."""
+        return [self.pipeline]
+
     def load_captioner(self) -> None:
         """loop.py:119-129: --captioner none -> no caption, ram -> RAM++ tags, llava -> a LLaVA-1.5 description, each
-        on the engine."""
-        if self.args.captioner == "llava":
+        on the engine. A rank that leaves captions to rank 0 loads none."""
+        if self.ranks is not None and not self.ranks.captions:
+            self.captioner = EmptyCaptioner(self.args.device)
+        elif self.args.captioner == "llava":
             from ..utils.caption import LLaVACaptioner
             self.captioner = LLaVACaptioner(self.args.device, self.args.llava_bit, self.weights_dir, self.synthetic,
                                             self.args.seed)
@@ -192,15 +201,22 @@ class InferenceLoop:
     def load_lq(self) -> Generator[Image.Image, None, None]:
         img_exts = [".png", ".jpg", ".jpeg"]
         assert os.path.isdir(self.args.input), "Please put your low-quality images in a folder."
+        k = -1
         for file_name in sorted(os.listdir(self.args.input)):
             stem, ext = os.path.splitext(file_name)
             if ext not in img_exts:
                 print(f"{file_name} is not an image, continue")
                 continue
+            k += 1
+            if self.ranks is not None and not self.ranks.takes(k):
+                continue
             file_path = os.path.join(self.args.input, file_name)
             lq = Image.open(file_path).convert("RGB")
             print(f"load lq: {file_path}")
             self.loop_ctx["file_stem"] = stem
+            self.loop_ctx["image_index"] = k
+            if self.ranks is not None:
+                self.ranks.start_image(k)
             yield lq
 
     def after_load_lq(self, lq: Image.Image) -> np.ndarray:
@@ -212,7 +228,8 @@ class InferenceLoop:
         a = self.args
         self.setup()
         for lq in self.load_lq():
-            caption = self.captioner(lq)                 # fp32 logits; nothing here runs under autocast
+            # fp32 logits; nothing here runs under autocast
+            caption = self.captioner(lq) if self.ranks is None else self.ranks.caption(self.captioner, lq)
             pos_prompt = prompt_with_caption(caption, a.pos_prompt)
             neg_prompt = a.neg_prompt
             lq = self.after_load_lq(lq)
@@ -228,7 +245,10 @@ class InferenceLoop:
                     a.cfg_scale, a.start_point_type, a.sampler, a.noise_aug, a.rescale_cfg, a.s_churn, a.s_tmin,
                     a.s_tmax, a.s_noise, a.eta, a.order)
                 samples.extend(list(batch_samples))
-            self.save(samples, pos_prompt, neg_prompt)
+            if self.ranks is None or self.ranks.writes:
+                self.save(samples, pos_prompt, neg_prompt)
+        if self.ranks is not None:
+            self.ranks.finish(self.save_dir)
 
     def save(self, samples: List[np.ndarray], pos_prompt: str, neg_prompt: str) -> None:
         file_stem = self.loop_ctx["file_stem"]
@@ -238,7 +258,14 @@ class InferenceLoop:
             save_path = os.path.join(self.save_dir, file_name)
             Image.fromarray(sample).save(save_path)
             print(f"save result to {save_path}")
-        append_prompt_row(self.save_dir, file_stem, pos_prompt, neg_prompt)
+        self.prompt_row(file_stem, pos_prompt, neg_prompt)
+
+    def prompt_row(self, file_stem: str, pos_prompt: str, neg_prompt: str) -> None:
+        """The prompt.csv row of the current input (under torchrun rank 0 writes them all, in input order)."""
+        if self.ranks is None:
+            append_prompt_row(self.save_dir, file_stem, pos_prompt, neg_prompt)
+        else:
+            self.ranks.prompt_row(self.save_dir, self.loop_ctx["image_index"], file_stem, pos_prompt, neg_prompt)
 
 
 def append_prompt_row(save_dir: str, file_stem: str, pos_prompt: str, neg_prompt: str) -> None:

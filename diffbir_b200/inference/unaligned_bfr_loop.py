@@ -14,7 +14,7 @@ from PIL import Image
 from ..pipeline import BSRNetPipeline, SwinIRPipeline
 from ..utils.common import instantiate_from_config
 from ..utils.face import FaceRestoreHelper
-from .loop import InferenceLoop, append_prompt_row, load_checkpoint, load_config
+from .loop import InferenceLoop, load_checkpoint, load_config
 from .pretrained_models import resolve
 
 
@@ -49,6 +49,9 @@ class UnAlignedBFRInferenceLoop(InferenceLoop):
             self.bg_requires_upscale = True
         self.pipeline_dict = {"background": bg,
                               "face": SwinIRPipeline(self.face_cleaner, self.cldm, self.diffusion, self.cond_fn, a.device)}
+
+    def pipelines(self) -> list:
+        return list(self.pipeline_dict.values())
 
     def face_networks(self):
         """(detector, parser) callables of FaceRestoreHelper, on the engines."""
@@ -108,8 +111,7 @@ class UnAlignedBFRInferenceLoop(InferenceLoop):
         import os
         stem = self.loop_ctx["file_stem"]
         is_face = self.loop_ctx["is_face"]
-        append_prompt_row(self.save_dir, f"{stem}_face_{self.loop_ctx['face_idx']}" if is_face else stem,
-                          pos_prompt, neg_prompt)
+        self.prompt_row(f"{stem}_face_{self.loop_ctx['face_idx']}" if is_face else stem, pos_prompt, neg_prompt)
         if is_face:
             face_idx = self.loop_ctx["face_idx"]
             for i, sample in enumerate(samples):

@@ -49,6 +49,9 @@ class ControlLDM:
         # tiled (all ranks must pass the same tensors; set by the pipeline while ranks cooperate on one job: tiled /
         # batch-sharded sampling)
         self.shard_vae = False
+        # False: while shard_vae is set, an un-tiled VAE stays replicated instead of row-sharded; the row-sharded one
+        # agrees with one GPU only to the fp16 noise floor, the tile-sharded one bit for bit
+        self.shard_vae_rows = True
         self._svae = None
         self._tvae = None
 
@@ -208,7 +211,7 @@ class ControlLDM:
 
     def _sharded_vae(self, h_img: int, w_img: int):
         """The row-sharded VAE (engine.vae_sharded) when ranks cooperate on this job and the size allows it."""
-        if not self.shard_vae:
+        if not (self.shard_vae and self.shard_vae_rows):
             return None
         from ..engine.vae_sharded import ShardedVae
         if not ShardedVae.usable(h_img, w_img):

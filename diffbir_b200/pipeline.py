@@ -65,6 +65,8 @@ class Pipeline:
         self.fused_post = True             # colour fix + quantisation as one kernel (False: the torch op sequence)
         self.shard_vae = True              # cooperating ranks (tiled / batch-sharded sampling) shard the VAE (by image rows or by tiles)
         self.shard_batch = False           # un-tiled batches: shard (image, CFG branch) forwards over torch.distributed ranks
+        self.shard_tiles = True            # tiled sampling: shard the tiles over torch.distributed ranks (Sampler.shard_tiles)
+        self.shard_cleaner = False         # stage 1 shared by the ranks: a tiled cleaner by windows, an un-tiled one on rank 0
         self.max_tile_forwards = 128       # tiled sampling: most tile-forwards x images per graph replay (Sampler.max_tile_forwards)
         self.marks: Optional[list] = None  # set to [] to record (phase, CUDA event) boundaries (bench.py phases_ms)
 
@@ -103,7 +105,8 @@ class Pipeline:
         # ranks that cooperate on this job (sharded tiles or batch units) also shard the VAE: the un-tiled one by
         # image rows, the tiled one by tiles (ControlLDM)
         import torch.distributed as dist
-        coop = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and (cldm_tiled or self.shard_batch)
+        coop = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and (
+            (cldm_tiled and self.shard_tiles) or self.shard_batch)
         self.cldm.shard_vae = bool(coop and self.shard_vae)
         # The reference encodes the (identical) condition image twice (pipeline.py:117-128);
         # the latent is deterministic (posterior mode), so it is encoded once and shared.
@@ -148,6 +151,7 @@ class Pipeline:
         else:
             raise NotImplementedError(sampler_type)
         sampler.shard_batch = self.shard_batch
+        sampler.shard_tiles = self.shard_tiles
         sampler.max_tile_forwards = self.max_tile_forwards
         if cldm_tiled and tiled_run_chunked(len(sliding_windows(h2, w2, cldm_tile_size // 8, cldm_tile_stride // 8)),
                                             1 if cfg_scale == 1.0 else 2, bs, self.max_tile_forwards,
@@ -209,7 +213,7 @@ class Pipeline:
         self._mark("start")
         lq_tensor = lq_dev.to(torch.float32).div(255).clamp(0, 1).permute(0, 3, 1, 2).contiguous()
         self.set_output_size(lq_tensor.size())
-        cond_img = self.apply_cleaner(lq_tensor, cleaner_tiled, cleaner_tile_size, cleaner_tile_stride)
+        cond_img = self.shared_cleaner(lq_tensor, cleaner_tiled, cleaner_tile_size, cleaner_tile_stride)
         self._mark("swinir")
         assert all(x >= 512 for x in cond_img.shape[2:]), (
             "The resolution of stage-1 model output should be greater than 512, "
@@ -238,6 +242,24 @@ class Pipeline:
         return out
 
 
+    def shared_cleaner(self, lq: torch.Tensor, tiled: bool, tile_size: int, tile_stride: int) -> torch.Tensor:
+        """apply_cleaner. With shard_cleaner set and more than one torch.distributed rank, every rank passes the same
+        input and gets the same stage-1 output: a tiled cleaner runs each rank's share of the windows (make_tiled_fn's
+        shard), an un-tiled one runs on rank 0, which broadcasts its output."""
+        import torch.distributed as dist
+        if not (self.shard_cleaner and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+            return self.apply_cleaner(lq, tiled, tile_size, tile_stride)
+        if tiled and lq.size(2) >= tile_size and lq.size(3) >= tile_size:       # apply_cleaner's own test for tiling
+            return self.apply_cleaner(lq, tiled, tile_size, tile_stride)
+        out = self.apply_cleaner(lq, tiled, tile_size, tile_stride).contiguous() if dist.get_rank() == 0 else None
+        meta = [(tuple(out.shape), out.dtype) if out is not None else None]
+        dist.broadcast_object_list(meta, src=0)
+        if out is None:
+            out = torch.empty(meta[0][0], dtype=meta[0][1], device=lq.device)
+        dist.broadcast(out, src=0)
+        return out
+
+
 class SwinIRPipeline(Pipeline):
     def apply_cleaner(self, lq: torch.Tensor, tiled: bool, tile_size: int, tile_stride: int) -> torch.Tensor:
         """pipeline.py:371-397. Un-tiled: resize the short edge to >= 512 first, pad to x64, crop.
@@ -255,7 +277,7 @@ class SwinIRPipeline(Pipeline):
             h0, w0 = lq.shape[2:]
             lq = pad_to_multiples_of(lq, multiple=64)
             return self.cleaner(lq)[:, :, :h0, :w0]
-        output = make_tiled_fn(self.cleaner, size=tile_size, stride=tile_stride)(lq)
+        output = make_tiled_fn(self.cleaner, size=tile_size, stride=tile_stride, shard=self.shard_cleaner)(lq)
         if min(output.shape[2:]) < 512:
             output = resize_short_edge_to(output, size=512)
         return output
@@ -277,7 +299,8 @@ class BSRNetPipeline(Pipeline):
         if tiled and (lq.size(2) < tile_size or lq.size(3) < tile_size):
             print("[BSRNet]: the input size is tiny and unnecessary to tile.")
             tiled = False
-        model = make_tiled_fn(self.cleaner, tile_size, tile_stride, scale_type="up", scale=4) if tiled else self.cleaner
+        model = make_tiled_fn(self.cleaner, tile_size, tile_stride, scale_type="up", scale=4,
+                                                  shard=self.shard_cleaner) if tiled else self.cleaner
         up4 = model(lq)
         if min(self.output_size) < 512:
             return resize_short_edge_to(up4, size=512)
@@ -292,7 +315,7 @@ class SCUNetPipeline(Pipeline):
         if tiled and (lq.size(2) < tile_size or lq.size(3) < tile_size):
             print("[SCUNet]: the input size is tiny and unnecessary to tile.")
             tiled = False
-        model = make_tiled_fn(self.cleaner, tile_size, tile_stride) if tiled else self.cleaner
+        model = make_tiled_fn(self.cleaner, tile_size, tile_stride, shard=self.shard_cleaner) if tiled else self.cleaner
         output = model(lq)
         if min(output.shape[2:]) < 512:
             output = resize_short_edge_to(output, size=512)

@@ -46,11 +46,16 @@ def gaussian_weights(tile_width: int, tile_height: int) -> np.ndarray:
 
 
 def make_tiled_fn(fn, size: int, stride: int, scale_type: str = "up", scale: int = 1, channel=None,
-                  weight: str = "gaussian", dtype=None, device=None, progress: bool = False):
+                  weight: str = "gaussian", dtype=None, device=None, progress: bool = False, shard: bool = False):
     """Image-tiling wrapper of utils/common.py:172-232: the first argument is cut into row-major
     `size` x `size` windows (last one snapped to the border), `fn(tile) * w` and `w` are accumulated
     in that order, the result is `out / count`. Weights are built in fp64 and cast to the output
-    dtype exactly like the reference; extra arguments get the window as hi/hi_end/wi/wi_end."""
+    dtype exactly like the reference; extra arguments get the window as hi/hi_end/wi/wi_end.
+
+    shard: with a torch.distributed group of more than one rank, every rank passes the same input, runs
+    the windows it owns (window t belongs to rank t % world), and one all-gather hands every rank all
+    window outputs, which it blends in the order above: the result is bit-identical to one rank's. `fn`
+    must return the output dtype."""
     def tiled_fn(x: torch.Tensor, *args, **kwargs) -> torch.Tensor:
         sc = (lambda n: int(n * scale)) if scale_type == "up" else (lambda n: int(n // scale))
         b, c, h, w = x.size()
@@ -60,11 +65,30 @@ def make_tiled_fn(fn, size: int, stride: int, scale_type: str = "up", scale: int
         ws = sc(size)
         wnp = gaussian_weights(ws, ws)[None, None] if weight == "gaussian" else np.ones((1, 1, ws, ws))
         weights = torch.tensor(wnp, dtype=out_dtype, device=out_device)
-        for hi, hi_end, wi, wi_end in sliding_windows(h, w, size, stride):
-            oh, oh_end, ow, ow_end = map(sc, (hi, hi_end, wi, wi_end))
+        wins = sliding_windows(h, w, size, stride)
+
+        def run(t):
+            hi, hi_end, wi, wi_end = wins[t]
             if len(args) or len(kwargs):
                 kwargs.update(dict(hi=hi, hi_end=hi_end, wi=wi, wi_end=wi_end))
-            out[..., oh:oh_end, ow:ow_end] += fn(x[..., hi:hi_end, wi:wi_end], *args, **kwargs) * weights
+            return fn(x[..., hi:hi_end, wi:wi_end], *args, **kwargs)
+
+        import torch.distributed as dist
+        shared = None
+        if shard and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            from ..sampler.sampler import tile_slots, tiles_of_rank
+            world, slots = dist.get_world_size(), tile_slots(len(wins), dist.get_world_size())
+            send = torch.zeros((slots, b, channel or c, ws, ws), dtype=out_dtype, device=out_device)
+            for s, t in enumerate(tiles_of_rank(len(wins), dist.get_rank(), world)):
+                send[s] = run(t)
+            # one buffer of every rank's slots (rank-major); ranks without a window still send their zero slots
+            shared = torch.empty((world * slots,) + tuple(send.shape[1:]), dtype=out_dtype, device=out_device)
+            dist.all_gather_into_tensor(shared, send)
+            del send
+        for t, (hi, hi_end, wi, wi_end) in enumerate(wins):
+            oh, oh_end, ow, ow_end = map(sc, (hi, hi_end, wi, wi_end))
+            y = run(t) if shared is None else shared[(t % world) * slots + t // world]     # window t: rank t % world
+            out[..., oh:oh_end, ow:ow_end] += y * weights
             count[..., oh:oh_end, ow:ow_end] += weights
         return out / count
 

@@ -8,7 +8,23 @@ Differences from the reference (each refused with a message, never silently igno
 read from --weights_dir (no downloads), `--synthetic` runs random-init weights of the real
 architecture, the defaults of --sampler / --captioner are the ones this package runs ("spaced",
 "none"), and tasks / samplers / captioners whose networks are outside the accelerated path raise
-NotImplementedError (diffbir_b200/inference/loop.py:check_supported)."""
+NotImplementedError (diffbir_b200/inference/loop.py:check_supported).
+
+Under torchrun (one process per GPU of the box) `--distribute` picks how the ranks share the work:
+
+  torchrun --nproc-per-node 8 inference.py --distribute images ...     # a folder: images dealt round-robin
+  torchrun --nproc-per-node 8 inference.py --distribute cooperate ...  # one large image: all GPUs on every image
+
+images: rank r restores the r-th, (r + W)-th, ... of the sorted input images and writes their PNGs; rank 0 writes
+prompt.csv, in input order and in the single-process format. Seed rule: image k (its index in the sorted list) is
+restored right after set_seed(seed + k), so each output is the same at every world size. This differs from the
+plain `python inference.py` run for k >= 1, which seeds once and lets image k's noise follow the images before it.
+cooperate: seeded once, as the single-process run, whose files with DBIR_DETERMINISTIC=1 it writes (from rank 0)
+bit for bit (without it the single-process plans may differ by one uint8 level): the prompt
+comes from rank 0's captioner, stage 1 is sharded by windows (--cleaner_tiled) or runs on rank 0, sampling is
+sharded by tiles (--cldm_tiled) or by (image, CFG branch) forwards, so at most 2 x --batch_size ranks work on an
+un-tiled image and the others idle. Under torchrun every engine selects its kernel plans independently of the
+process (diffbir_b200/inference/ranks.py). Without torchrun's variables nothing here uses torch.distributed."""
 import random
 from argparse import ArgumentParser, Namespace
 
@@ -82,6 +98,9 @@ def build_parser() -> ArgumentParser:
     # this package only
     p.add_argument("--weights_dir", type=str, default="", help="Directory holding the reference's checkpoint files.")
     p.add_argument("--synthetic", action="store_true", help="Random-init weights of the real architecture.")
+    p.add_argument("--distribute", type=str, default="images", choices=["images", "cooperate"],
+                   help="Under torchrun: deal the images over the GPUs (images) or run every image on all of them "
+                        "(cooperate). Ignored otherwise.")
     return p
 
 
@@ -102,15 +121,24 @@ def main(argv=None) -> None:
     args = parse_args(argv)
     if args.device == "cuda" and not torch.cuda.is_available():
         raise SystemExit("inference.py needs a CUDA device (sm_90a): there is no CPU fallback for the engines")
-    set_seed(args.seed)
-    from diffbir_b200.inference import (BFRInferenceLoop, BIDInferenceLoop, BSRInferenceLoop, CustomInferenceLoop,
-                                        UnAlignedBFRInferenceLoop)
-    loops = {"sr": BSRInferenceLoop, "face": BFRInferenceLoop, "denoise": BIDInferenceLoop,
-             "unaligned_face": UnAlignedBFRInferenceLoop}
-    if args.version == "custom":
-        CustomInferenceLoop(args).run()
-    else:
-        loops[args.task](args).run()
+    from diffbir_b200.inference import ranks as rank_mod
+    ranks = rank_mod.launch(args, set_seed)
+    try:
+        set_seed(args.seed)
+        from diffbir_b200.inference import (BFRInferenceLoop, BIDInferenceLoop, BSRInferenceLoop, CustomInferenceLoop,
+                                            UnAlignedBFRInferenceLoop)
+        loops = {"sr": BSRInferenceLoop, "face": BFRInferenceLoop, "denoise": BIDInferenceLoop,
+                 "unaligned_face": UnAlignedBFRInferenceLoop}
+        cls = CustomInferenceLoop if args.version == "custom" else loops[args.task]
+        if ranks is None:
+            loop = cls(args)
+        else:
+            loop = cls(args, ranks)
+            ranks.configure(loop.pipelines())
+        loop.run()
+    finally:
+        if ranks is not None:
+            rank_mod.close()
     print("done!")
 
 
