@@ -466,3 +466,83 @@ def embed_gather(table, vocab, ids, n, dim, out, ldo):
     check(load().dbir_embed_gather(_fp(table), vocab, _fp(ids), n, dim, _fp(out), C.c_int64(ldo), _sp()),
           "dbir_embed_gather")
     count_launch()
+
+
+# ---- Real-ESRGAN degradation (include/diffbir_b200.h, "Real-ESRGAN degradation") ----
+RESIZE_MODE = {"area": 0, "bilinear": 1, "bicubic": 2}
+
+
+def filter2d(x, kernel, out, *, sub=None, threshold=0.0):
+    """out = filter2D(x, kernel) (reflect padding); kernel [1 or b, k, k]. sub: filter the mask |x - sub|*255 > threshold."""
+    b, c, h, w = x.shape
+    k = kernel.shape[-1]
+    stride = 0 if kernel.shape[0] == 1 else k * k
+    check(load().dbir_filter2d(_fp(x), _fp(sub), C.c_float(threshold), b, c, h, w, _fp(kernel), C.c_int64(stride), k,
+                               _fp(out), _sp()), "dbir_filter2d")
+    count_launch()
+
+
+def resize(x, out, mode, ratio_h, ratio_w):
+    """F.interpolate(x, ...) into out (align_corners=False); ratio = source / destination coordinate scale."""
+    b, c, hin, win = x.shape
+    check(load().dbir_resize(_fp(x), C.c_int64(b * c), hin, win, out.shape[2], out.shape[3], RESIZE_MODE[mode],
+                             C.c_float(ratio_h), C.c_float(ratio_w), _fp(out), _sp()), "dbir_resize")
+    count_launch()
+
+
+def gaussian_noise(img, noise, noise_gray, u_sigma, sigma_lo, sigma_span, u_gray, gray_prob, out):
+    b, c, h, w = img.shape
+    check(load().dbir_gaussian_noise(_fp(img), _fp(noise), _fp(noise_gray), _fp(u_sigma), C.c_float(sigma_lo),
+                                     C.c_float(sigma_span), _fp(u_gray), C.c_float(gray_prob), b, c, C.c_int64(h * w),
+                                     _fp(out), _sp()), "dbir_gaussian_noise")
+    count_launch()
+
+
+def noise_levels(img, q, hist, *, gray=False):
+    b, c, h, w = img.shape
+    check(load().dbir_noise_levels(_fp(img), b, c, C.c_int64(h * w), 1 if gray else 0, _fp(q), _fp(hist), _sp()),
+          "dbir_noise_levels")
+    count_launch()
+
+
+def poisson_rate(q, hist, vals, rate):
+    b = q.shape[0]
+    check(load().dbir_poisson_rate(_fp(q), _fp(hist), b, C.c_int64(q[0].numel()), _fp(vals), _fp(rate), _sp()),
+          "dbir_poisson_rate")
+    count_launch()
+
+
+def poisson_noise(img, q, draw, vals, u_scale, scale_lo, scale_span, out, *, q_gray=None, draw_gray=None,
+                  vals_gray=None, u_gray=None, gray_prob=0.0):
+    b, c, h, w = img.shape
+    check(load().dbir_poisson_noise(_fp(img), _fp(q), _fp(draw), _fp(vals), _fp(q_gray), _fp(draw_gray),
+                                    _fp(vals_gray), _fp(u_scale), C.c_float(scale_lo), C.c_float(scale_span),
+                                    _fp(u_gray), C.c_float(gray_prob), b, c, C.c_int64(h * w), _fp(out), _sp()),
+          "dbir_poisson_noise")
+    count_launch()
+
+
+def diffjpeg(x, quality, out, *, clamp_in=False, is_factor=False):
+    """quality [b]: qualities, or (is_factor=True) the table factors themselves."""
+    b, c, h, w = x.shape
+    check(load().dbir_diffjpeg(_fp(x), _fp(quality), 1 if is_factor else 0, b, h, w, 1 if clamp_in else 0, _fp(out),
+                               _sp()), "dbir_diffjpeg")
+    count_launch()
+
+
+def usm_blend(img, blur, soft, weight, out):
+    check(load().dbir_usm_blend(_fp(img), _fp(blur), _fp(soft), C.c_float(weight), C.c_int64(img.numel()), _fp(out),
+                                _sp()), "dbir_usm_blend")
+    count_launch()
+
+
+def lq_levels(x, out):
+    check(load().dbir_lq_levels(_fp(x), C.c_int64(x.numel()), _fp(out), _sp()), "dbir_lq_levels")
+    count_launch()
+
+
+def pair_nhwc(lq, hq, lq_out, hq_out):
+    b, c, h, w = lq.shape
+    check(load().dbir_pair_nhwc(_fp(lq), _fp(hq), b, c, C.c_int64(h * w), _fp(lq_out), _fp(hq_out), _sp()),
+          "dbir_pair_nhwc")
+    count_launch()

@@ -307,6 +307,53 @@ int dbir_wavelet_fix(const float* sample, int64_t s_img, int64_t s_ch, int64_t s
                      const float* style, int64_t t_img, int64_t t_ch, int64_t t_row,
                      int32_t batch, int32_t h, int32_t w, void* out_u8, float* out_f32, void* stream);
 
+/* ---- Real-ESRGAN degradation (dataset/batch_transform.py:142-285) -----------------------------
+ * fp32 NCHW in and out, contiguous. The random draws stay with the caller (torch generators); these
+ * entries compute what lies between them. Per-sample parameters are passed as the raw uniform draws u
+ * with param = u * span + lo and gray = (u_gray < gray_prob), evaluated on the device.
+ * filter2d: utils.py:162-187, reflect padding, odd k <= 63, h and w > k/2. kernel [kb, k, k] with
+ *   kernel_stride = k*k (one per sample) or 0 (one for the batch). sub != NULL filters the USM threshold
+ *   mask (|x - sub| * 255 > threshold) instead of x (utils.py:205-207).
+ * resize: F.interpolate, align_corners=False, no antialias; mode 0 area (adaptive_avg_pool2d bins),
+ *   1 bilinear, 2 bicubic (A = -0.75). ratio = source/destination coordinate scale: 1/scale_factor
+ *   for the scale_factor= form, in/out for the size= form.
+ * gaussian_noise: degradation.py:461-554; noise [b,c,h,w] and noise_gray [h,w] (or NULL) are torch.randn draws.
+ * noise_levels: q = clamp(round(x*255), 0, 255)/255 (gray = 1: of rgb_to_grayscale(x), one channel) and the
+ *   256-bin level histogram per sample, hist int32 [b, 256] (zeroed here).
+ * poisson_rate: vals[s] = 2^ceil(log2(distinct levels of sample s)), rate = q * vals (torch.poisson's input).
+ * poisson_noise: degradation.py:610-724: noise = draw/vals - q, mixed with the gray field's when q_gray != NULL,
+ *   times the scale; out = clip(img + noise, 0, 1).
+ * diffjpeg: diffjpeg.py:450-492 with differentiable=False; quality [b]: with quality_is_factor = 0 the quality of
+ *   each sample, turned into its table factor on the device as PyTorch does for a tensor quality; with 1 the factors
+ *   themselves (a Python-number quality, whose factor the reference computes in double on the host).
+ *   clamp_in = 1 clamps the input to [0, 1] first (batch_transform.py:192,255,260).
+ * usm_blend: utils.py:208-210, soft = filter2d of the threshold mask.
+ * lq_levels: clamp(round(x*255), 0, 255)/255 (batch_transform.py:271).
+ * pair_nhwc: lq -> NHWC, hq*2-1 -> NHWC (batch_transform.py:279-281).
+ */
+int dbir_filter2d(const float* x, const float* sub, float threshold, int32_t b, int32_t c, int32_t h, int32_t w,
+                  const float* kernel, int64_t kernel_stride, int32_t k, float* out, void* stream);
+int dbir_resize(const float* x, int64_t planes, int32_t hin, int32_t win, int32_t hout, int32_t wout, int32_t mode,
+                float ratio_h, float ratio_w, float* out, void* stream);
+int dbir_gaussian_noise(const float* img, const float* noise, const float* noise_gray, const float* u_sigma,
+                        float sigma_lo, float sigma_span, const float* u_gray, float gray_prob, int32_t b, int32_t c,
+                        int64_t hw, float* out, void* stream);
+int dbir_noise_levels(const float* img, int32_t b, int32_t c, int64_t hw, int32_t gray, float* q, int32_t* hist,
+                      void* stream);
+int dbir_poisson_rate(const float* q, const int32_t* hist, int32_t b, int64_t per_sample, float* vals, float* rate,
+                      void* stream);
+int dbir_poisson_noise(const float* img, const float* q, const float* draw, const float* vals, const float* q_gray,
+                       const float* draw_gray, const float* vals_gray, const float* u_scale, float scale_lo,
+                       float scale_span, const float* u_gray, float gray_prob, int32_t b, int32_t c, int64_t hw,
+                       float* out, void* stream);
+int dbir_diffjpeg(const float* x, const float* quality, int32_t quality_is_factor, int32_t b, int32_t h, int32_t w,
+                  int32_t clamp_in, float* out, void* stream);
+int dbir_usm_blend(const float* img, const float* blur, const float* soft, float weight, int64_t n, float* out,
+                   void* stream);
+int dbir_lq_levels(const float* x, int64_t n, float* out, void* stream);
+int dbir_pair_nhwc(const float* lq, const float* hq, int32_t b, int32_t c, int64_t hw, float* lq_out, float* hq_out,
+                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif
