@@ -546,3 +546,19 @@ def pair_nhwc(lq, hq, lq_out, hq_out):
     check(load().dbir_pair_nhwc(_fp(lq), _fp(hq), b, c, C.c_int64(h * w), _fp(lq_out), _fp(hq_out), _sp()),
           "dbir_pair_nhwc")
     count_launch()
+
+
+# ---- Brownian tree (include/diffbir_b200.h, "Brownian tree") ----
+def brownian_increment(out, seed, lo, hi, t0, t1, depth):
+    """out (fp32, contiguous, on the device) = W(t1) - W(t0) per element of the seeded Brownian tree on [lo, hi]."""
+    check(load().dbir_brownian_increment(_fp(out), C.c_int64(out.numel()), C.c_uint64(seed), C.c_double(lo),
+                                         C.c_double(hi), C.c_double(t0), C.c_double(t1), depth, _sp()),
+          "dbir_brownian_increment")
+    count_launch()
+
+
+def brownian_draws(n, seed, node, *, leaf=False, t=0.0, words=None, normals=None):
+    """The tree's raw draws at one node (or the leaf draw at t): words uint32 [n, 4] (as int32), normals fp64 [n]."""
+    check(load().dbir_brownian_draws(_fp(words), _fp(normals), C.c_int64(n), C.c_uint64(seed), C.c_uint64(node),
+                                     1 if leaf else 0, C.c_double(t), _sp()), "dbir_brownian_draws")
+    count_launch()

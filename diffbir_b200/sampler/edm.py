@@ -14,8 +14,11 @@ fixtures the reference produced).
 Stochastic "SDE" rules draw their noise from torchsde's Brownian tree in the reference
 (k_diffusion.py:70-120). torchsde is not a dependency here: when it is importable the same tree is used,
 otherwise `dpm++_2m_sde` / `dpm++_3m_sde` (one query per step, disjoint intervals => independent standard
-normals, the same distribution) fall back to torch.randn_like and `dpm++_sde` (overlapping intervals)
-is refused.
+normals, the same distribution) fall back to torch.randn_like, and `dpm++_sde` (two overlapping intervals per
+step, whose increments must come from one path) queries `DeviceBrownianTree`: a Brownian tree the engine generates
+on the fly from (seed, node, element) (dbir_brownian_increment), with torchsde's tolerance and k-diffusion's
+interface (same seed draw, interval [min sigma > 0, max sigma], sign rule and scaling). It has torchsde's
+distribution and query semantics, not its random stream.
 """
 from __future__ import annotations
 
@@ -291,19 +294,55 @@ STEP_RULES: Dict[str, Tuple[Callable, Tuple[str, ...], Optional[str]]] = {
 _DISJOINT_QUERIES = {"dpm++_2m_sde", "dpm++_3m_sde"}       # one noise query per step over [sigma_i+1, sigma_i]
 
 
+BROWNIAN_TOL = 1e-6            # torchsde.BrownianTree's default tolerance: the widest leaf of the tree
+
+
+def brownian_depth(lo: float, hi: float, tol: float = BROWNIAN_TOL) -> int:
+    """Fewest bisections of [lo, hi] that leave leaves no wider than `tol` (34 for the v2 / v2.1 ladders, whose
+    sigma_max is about 1e4)."""
+    d = 0
+    while (hi - lo) / 2.0 ** d > tol:
+        d += 1
+    return d
+
+
+class DeviceBrownianTree:
+    """torchsde.BrownianTree(lo, zeros_like(x), hi, entropy=seed) as the engine builds it: `tree(t0, t1)` is
+    W(t1) - W(t0) for every element of x, computed by one dbir_brownian_increment launch from (seed, node, element)
+    alone. No tree is stored: the same query gives the same bits every time, and an element's value does not depend
+    on the size of x."""
+
+    def __init__(self, x: torch.Tensor, lo, hi, seed: int):
+        if not x.is_cuda:
+            raise ValueError("the device Brownian tree of edm_dpm++_sde needs a CUDA latent (install torchsde to "
+                             "sample on another device)")
+        self.shape, self.device = x.shape, x.device
+        self.lo, self.hi, self.seed = float(lo), float(hi), int(seed)
+        self.depth = brownian_depth(self.lo, self.hi)
+
+    def __call__(self, t0, t1) -> torch.Tensor:
+        from .. import lib
+        out = torch.empty(self.shape, dtype=torch.float32, device=self.device)
+        lib.brownian_increment(out, self.seed, self.lo, self.hi, float(t0), float(t1), self.depth)
+        return out
+
+
 def _brownian_noise(x: torch.Tensor, sigmas: torch.Tensor, solver: str) -> Optional[Callable]:
-    """BrownianTreeNoiseSampler(x, sigma_min, sigma_max) (k_diffusion.py:97-120) when torchsde is there."""
+    """BrownianTreeNoiseSampler(x, sigma_min, sigma_max) (k_diffusion.py:97-120) on torchsde's tree when torchsde is
+    there, else on DeviceBrownianTree. The seed comes from the CPU generator, as in k-diffusion; ranks that cooperate
+    on one image are all seeded alike and make the same CPU draws before this one, so they draw the same seed."""
     try:
         import torchsde
     except ImportError:
         if solver in _DISJOINT_QUERIES:
             return None                                     # independent N(0, I) draws: same distribution
-        raise NotImplementedError(
-            f"edm_{solver} queries overlapping Brownian intervals and needs the torchsde package "
-            "(k_diffusion.py:70-120); use edm_dpm++_2m_sde / edm_dpm++_3m_sde or install torchsde")
+        torchsde = None
     lo, hi = torch.as_tensor(sigmas[sigmas > 0].min()), torch.as_tensor(sigmas.max())
     seed = torch.randint(0, 2 ** 63 - 1, []).item()
-    tree = torchsde.BrownianTree(lo, torch.zeros_like(x), hi, entropy=seed)
+    if torchsde is None:
+        tree = DeviceBrownianTree(x, lo, hi, seed)
+    else:
+        tree = torchsde.BrownianTree(lo, torch.zeros_like(x), hi, entropy=seed)
 
     def sample(s0, s1):
         a, b = torch.as_tensor(s0), torch.as_tensor(s1)

@@ -354,6 +354,23 @@ int dbir_lq_levels(const float* x, int64_t n, float* out, void* stream);
 int dbir_pair_nhwc(const float* lq, const float* hq, int32_t b, int32_t c, int64_t hw, float* lq_out, float* hq_out,
                    void* stream);
 
+/* ---- Brownian tree (noise of the dpm++_sde step rule, sampler/k_diffusion.py:70-120, 548-586) ----------------
+ * brownian_increment: out[e] = W_e(t1) - W_e(t0) (fp32) for e < n, where W_e is a Brownian motion on [lo, hi] with
+ *   W_e(lo) = 0, the same for every call with the same (seed, lo, hi, depth). W(t) walks `depth` levels of the dyadic
+ *   bisection of [lo, hi]: each midpoint is a Brownian-bridge draw between its interval's end values, and below the
+ *   last level W(t) is one more bridge draw between the leaf's ends, keyed with t. t0 and t1 are clamped to [lo, hi].
+ *   Every draw is a Philox4x32-10 normal (Box-Muller) keyed by (seed, node, element); the walk runs in fp64.
+ *   0 <= depth <= 62; pick it so that (hi - lo) / 2^depth is the tolerance wanted.
+ * brownian_draws: the raw draws that walk uses, for checking the stream: for e < n, the four Philox words
+ *   (words_out uint32 [n, 4]) and the normal (normals fp64 [n]) of element e at `node` (heap numbering: 0 is W(hi),
+ *   1 the midpoint of [lo, hi], 2k and 2k + 1 the midpoints of node k's halves), or with leaf = 1 of the leaf draw
+ *   at time t. Either output may be NULL.
+ */
+int dbir_brownian_increment(float* out, int64_t n, uint64_t seed, double lo, double hi, double t0, double t1,
+                            int32_t depth, void* stream);
+int dbir_brownian_draws(uint32_t* words_out, double* normals, int64_t n, uint64_t seed, uint64_t node, int32_t leaf,
+                        double t, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
