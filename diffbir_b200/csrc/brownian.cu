@@ -74,11 +74,9 @@ struct Walk {
   }
 };
 
-__global__ void __launch_bounds__(THREADS)
-brownian_increment_kernel(float* __restrict__ out, long long n, unsigned long long seed, double lo, double hi,
-                          double t0, double t1, int depth) {
-  const long long e = static_cast<long long>(blockIdx.x) * THREADS + threadIdx.x;
-  if (e >= n) return;
+// W(t1) - W(t0) of element e of the tree seeded `seed`
+__device__ __forceinline__ float increment(long long e, unsigned long long seed, double lo, double hi, double t0,
+                                           double t1, int depth) {
   const Key k{static_cast<uint32_t>(e), static_cast<uint32_t>(e >> 32), seed};
   t0 = fmin(fmax(t0, lo), hi);
   t1 = fmin(fmax(t1, lo), hi);
@@ -93,7 +91,25 @@ brownian_increment_kernel(float* __restrict__ out, long long n, unsigned long lo
   }
   const double w0 = bridge(p.a, p.b, p.wa, p.wb, t0, box_muller(words(k, p.node, true, t0)));
   const double w1 = bridge(q.a, q.b, q.wa, q.wb, t1, box_muller(words(k, q.node, true, t1)));
-  out[e] = static_cast<float>(w1 - w0);
+  return static_cast<float>(w1 - w0);
+}
+
+__global__ void __launch_bounds__(THREADS)
+brownian_increment_kernel(float* __restrict__ out, long long n, unsigned long long seed, double lo, double hi,
+                          double t0, double t1, int depth) {
+  const long long e = static_cast<long long>(blockIdx.x) * THREADS + threadIdx.x;
+  if (e >= n) return;
+  out[e] = increment(e, seed, lo, hi, t0, t1, depth);
+}
+
+// one tree per sample: element e of sample b is element e of the tree seeded seeds[b]
+__global__ void __launch_bounds__(THREADS)
+brownian_increment_samples_kernel(float* __restrict__ out, long long n, const unsigned long long* __restrict__ seeds,
+                                  double lo, double hi, double t0, double t1, int depth) {
+  const long long e = static_cast<long long>(blockIdx.x) * THREADS + threadIdx.x;
+  const int b = blockIdx.y;
+  if (e >= n) return;
+  out[b * n + e] = increment(e, seeds[b], lo, hi, t0, t1, depth);
 }
 
 __global__ void __launch_bounds__(THREADS)
@@ -118,6 +134,18 @@ extern "C" int dbir_brownian_increment(float* out, int64_t n, uint64_t seed, dou
                depth);
   brownian_increment_kernel<<<blocks(n), THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       out, n, seed, lo, hi, t0, t1, depth);
+  DBIR_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dbir_brownian_increment_samples(float* out, int64_t n, int32_t samples, const uint64_t* seeds, double lo,
+                                               double hi, double t0, double t1, int32_t depth, void* stream) {
+  DBIR_REQUIRE(out && seeds && n > 0 && n <= (1LL << 31) * THREADS && samples > 0 && samples <= 65535,
+               "dbir_brownian_increment_samples: bad output (n = %lld, samples = %d)", static_cast<long long>(n), samples);
+  DBIR_REQUIRE(lo <= hi && depth >= 0 && depth <= 62, "dbir_brownian_increment_samples: bad tree [%g, %g], depth %d", lo,
+               hi, depth);
+  brownian_increment_samples_kernel<<<dim3(blocks(n), samples), THREADS, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      out, n, reinterpret_cast<const unsigned long long*>(seeds), lo, hi, t0, t1, depth);
   DBIR_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

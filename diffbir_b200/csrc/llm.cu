@@ -49,14 +49,19 @@ rmsnorm_kernel(const float* __restrict__ x, long long ldx, int c, const float* _
 }
 
 // RoPE (rotate_half form, LlamaRotaryEmbedding with base theta) on q and k of the fused QKV rows, in fp32, and the
-// cache write. Row i sits at position p0[0] + i. CTA (row, head), 64 threads: thread d rotates the pair (d, d + 64).
+// cache write. Row i sits at position p0[0] + i; with cache_stride > 0, row i is sequence i at position p0[0], whose
+// cache starts i * cache_stride elements in. CTA (row, head), 64 threads: thread d rotates the pair (d, d + 64).
 __global__ void __launch_bounds__(64)
 rope_kv_kernel(const float* __restrict__ qkv, long long ldqkv, int heads, const int* __restrict__ p0, float theta,
-               op_t* __restrict__ q, long long ldq, op_t* __restrict__ kc, op_t* __restrict__ vc) {
+               op_t* __restrict__ q, long long ldq, op_t* __restrict__ kc, op_t* __restrict__ vc, long long cache_stride) {
   pdl_trigger();
   pdl_wait();
   const int row = blockIdx.x, h = blockIdx.y, d = threadIdx.x;
-  const int pos = p0[0] + row;
+  const int pos = p0[0] + (cache_stride ? 0 : row);
+  if (cache_stride) {
+    kc += row * cache_stride;
+    vc += row * cache_stride;
+  }
   const float inv_freq = 1.0f / powf(theta, static_cast<float>(2 * d) / HD);
   float sn, cs;
   sincosf(static_cast<float>(pos) * inv_freq, &sn, &cs);
@@ -201,17 +206,23 @@ attention_causal_kernel(const op_t* __restrict__ q, long long ldq, const op_t* _
 // ---- decode-step attention: one query row per head against the first len[0] cache rows ----
 // Pass 1: CTA (head, split) takes keys [split * 64, split * 64 + 64) and writes its running max, sum of
 // exponentials and un-normalised output to the workspace; splits past the length exit. Pass 2: CTA per head
-// combines the splits in index order (deterministic).
+// combines the splits in index order (deterministic). Sequence b of a batch (blockIdx.z in pass 1, blockIdx.y in
+// pass 2) reads query row b, cache b and workspace slice b, so its bits do not depend on the batch.
 constexpr int DEC_CHUNK = 64;
 
 __global__ void __launch_bounds__(128)
-attention_decode_part_kernel(const op_t* __restrict__ q, const op_t* __restrict__ kc, const op_t* __restrict__ vc,
-                             int heads, const int* __restrict__ len, float* __restrict__ ws) {
+attention_decode_part_kernel(const op_t* __restrict__ q, long long ldq, const op_t* __restrict__ kc,
+                             const op_t* __restrict__ vc, long long cache_stride, int heads, const int* __restrict__ len,
+                             float* __restrict__ ws) {
   __shared__ float s_p[DEC_CHUNK];
   __shared__ float s_red[2];
   pdl_trigger();
   pdl_wait();
-  const int h = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y;
+  const int h = blockIdx.x, split = blockIdx.y, nsplit = gridDim.y, b = blockIdx.z;
+  q += b * ldq;
+  kc += b * cache_stride;
+  vc += b * cache_stride;
+  ws += static_cast<long long>(b) * heads * nsplit * (HD + 2);
   const int L = len[0];
   const int k0 = split * DEC_CHUNK;
   if (k0 >= L) return;
@@ -261,10 +272,12 @@ attention_decode_part_kernel(const op_t* __restrict__ q, const op_t* __restrict_
 
 __global__ void __launch_bounds__(128)
 attention_decode_combine_kernel(const float* __restrict__ ws, const int* __restrict__ len, int nsplit,
-                                op_t* __restrict__ out) {
+                                op_t* __restrict__ out, long long ldo) {
   pdl_trigger();
   pdl_wait();
-  const int h = blockIdx.x, tid = threadIdx.x;
+  const int h = blockIdx.x, tid = threadIdx.x, b = blockIdx.y;
+  ws += static_cast<long long>(b) * gridDim.x * nsplit * (HD + 2);
+  out += b * ldo;
   const int used = (len[0] + DEC_CHUNK - 1) / DEC_CHUNK;
   const float* w = ws + static_cast<long long>(h) * nsplit * (HD + 2);
   float m = -INFINITY;
@@ -278,72 +291,127 @@ attention_decode_combine_kernel(const float* __restrict__ ws, const int* __restr
   out[h * HD + tid] = f2op(acc / l);
 }
 
-// ---- y = W x for one input row (decode step) ----
-// One warp per output (SwiGLU: per value / gate row pair), 16-byte loads of the op16 weight row, fp32
-// accumulation in a fixed order (lane-strided partial sums, then a butterfly). x is read through L1.
+// ---- y = W x for R <= 8 input rows (decode step of R sequences) ----
+// A warp owns OUTS outputs (SwiGLU: value / gate row pairs). Per 16-byte chunk of its weight rows it loads and
+// unpacks each x row once and applies it to all OUTS outputs, so at R > 1 the x traffic through L1 and its unpacking
+// are shared instead of repeated per output; every weight row is read once for all R rows. Each (output, row) sum is
+// fp32 in a fixed order (lane-strided partial sums in k, then a butterfly), the same for every R and OUTS: the bits
+// of row r equal the single-row call's. R = 1 keeps one output per warp and 8 warps per CTA.
 // mode 0: y = Wx; 1: y = Wx + residual; 2: SwiGLU over rows packed per `pack`-row tile as [values | gates]:
 // y[c] = v(c) * silu(g(c)) with v / g the rows of c's tile (dbir_gemm's geglu = 2 packing).
-constexpr int GEMV_WARPS = 8;
+template <int MODE, int R>
+struct GemvShape {
+  static constexpr int OUTS = R == 1 ? 1 : (MODE == 2 ? 2 : 4);    // outputs per warp
+  static constexpr int WARPS = R == 1 ? 8 : 4;                      // warps per CTA
+  static constexpr int UNROLL = R == 1 ? 4 : 2;
+};
 
-template <int MODE>
-__global__ void __launch_bounds__(GEMV_WARPS * 32)
-gemv_kernel(const op_t* __restrict__ w, long long ldw, const op_t* __restrict__ x, int n_out, int K, int pack,
-            const float* residual, void* y, int out_kind) {
+template <int MODE, int R>
+__global__ void __launch_bounds__(GemvShape<MODE, R>::WARPS * 32)
+gemv_kernel(const op_t* __restrict__ w, long long ldw, const op_t* __restrict__ x, long long ldx, int n_out, int K,
+            int pack, const float* residual, long long ldr, void* y, long long ldy, int out_kind) {
+  constexpr int OUTS = GemvShape<MODE, R>::OUTS, WARPS = GemvShape<MODE, R>::WARPS;
   pdl_trigger();
   pdl_wait();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int c = blockIdx.x * GEMV_WARPS + warp;
-  if (c >= n_out) return;
-  long long ra = c, rb = 0;
-  if (MODE == 2) {
-    const int hb = pack / 2, t = c / hb, j = c % hb;
-    ra = static_cast<long long>(t) * pack + j;
-    rb = ra + hb;
-  }
-  const op_t* wa = w + ra * ldw;
-  const op_t* wb = w + rb * ldw;
-  float sa = 0.f, sb = 0.f;
-#pragma unroll 4
-  for (int k = lane * 8; k < K; k += 256) {
-    const uint4 xv = __ldg(reinterpret_cast<const uint4*>(x + k));
-    const uint4 av = __ldcs(reinterpret_cast<const uint4*>(wa + k));
-    const uint32_t* xw = reinterpret_cast<const uint32_t*>(&xv);
-    const uint32_t* aw = reinterpret_cast<const uint32_t*>(&av);
+  const int c0 = (blockIdx.x * WARPS + warp) * OUTS;
+  if (c0 >= n_out) return;
+  const op_t* wa[OUTS];
+  const op_t* wb[OUTS];
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float2 xf = unpack2(xw[e]), af = unpack2(aw[e]);
-      sa = fmaf(af.x, xf.x, sa);
-      sa = fmaf(af.y, xf.y, sa);
-    }
+  for (int o = 0; o < OUTS; ++o) {
+    const int c = min(c0 + o, n_out - 1);        // outputs past the end repeat the last one and are not stored
+    long long ra = c, rb = 0;
     if (MODE == 2) {
-      const uint4 bv = __ldcs(reinterpret_cast<const uint4*>(wb + k));
-      const uint32_t* bw = reinterpret_cast<const uint32_t*>(&bv);
+      const int hb = pack / 2, t = c / hb, j = c % hb;
+      ra = static_cast<long long>(t) * pack + j;
+      rb = ra + hb;
+    }
+    wa[o] = w + ra * ldw;
+    wb[o] = w + rb * ldw;
+  }
+  float sa[OUTS][R], sb[OUTS][R];
+#pragma unroll
+  for (int o = 0; o < OUTS; ++o)
+#pragma unroll
+    for (int r = 0; r < R; ++r) sa[o][r] = sb[o][r] = 0.f;
+#pragma unroll GemvShape<MODE, R>::UNROLL
+  for (int k = lane * 8; k < K; k += 256) {
+    float af[OUTS][8], bf[OUTS][8];
+#pragma unroll
+    for (int o = 0; o < OUTS; ++o) {
+      const uint4 av = __ldcs(reinterpret_cast<const uint4*>(wa[o] + k));
+      const uint32_t* aw = reinterpret_cast<const uint32_t*>(&av);
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float2 xf = unpack2(xw[e]), bf = unpack2(bw[e]);
-        sb = fmaf(bf.x, xf.x, sb);
-        sb = fmaf(bf.y, xf.y, sb);
+        const float2 f = unpack2(aw[e]);
+        af[o][2 * e] = f.x;
+        af[o][2 * e + 1] = f.y;
+      }
+      if (MODE == 2) {
+        const uint4 bv = __ldcs(reinterpret_cast<const uint4*>(wb[o] + k));
+        const uint32_t* bw = reinterpret_cast<const uint32_t*>(&bv);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float2 f = unpack2(bw[e]);
+          bf[o][2 * e] = f.x;
+          bf[o][2 * e + 1] = f.y;
+        }
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      const uint4 xv = __ldg(reinterpret_cast<const uint4*>(x + r * ldx + k));
+      const uint32_t* xw = reinterpret_cast<const uint32_t*>(&xv);
+      float xf[8];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float2 f = unpack2(xw[e]);
+        xf[2 * e] = f.x;
+        xf[2 * e + 1] = f.y;
+      }
+#pragma unroll
+      for (int o = 0; o < OUTS; ++o) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) sa[o][r] = fmaf(af[o][i], xf[i], sa[o][r]);
+        if (MODE == 2) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) sb[o][r] = fmaf(bf[o][i], xf[i], sb[o][r]);
+        }
       }
     }
   }
-  sa = warp_sum(sa);
-  if (MODE == 2) sb = warp_sum(sb);
-  if (lane == 0) {
-    float v = sa;
-    if (MODE == 1) v += residual[c];
-    if (MODE == 2) v = sa * silu_f(sb);
-    if (out_kind == 0) static_cast<float*>(y)[c] = v;
-    else static_cast<op_t*>(y)[c] = f2op(v);
+#pragma unroll
+  for (int o = 0; o < OUTS; ++o) {
+    const int c = c0 + o;
+    if (c >= n_out) break;                       // warp-uniform
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      sa[o][r] = warp_sum(sa[o][r]);
+      if (MODE == 2) sb[o][r] = warp_sum(sb[o][r]);
+      if (lane == 0) {
+        float v = sa[o][r];
+        if (MODE == 1) v += residual[r * ldr + c];
+        if (MODE == 2) v = sa[o][r] * silu_f(sb[o][r]);
+        if (out_kind == 0) static_cast<float*>(y)[r * ldy + c] = v;
+        else static_cast<op_t*>(y)[r * ldy + c] = f2op(v);
+      }
+    }
   }
 }
 
 // First maximum of n fp32 logits -> *token; then every advance[i] += 1 (the decode step's position / length).
+// CTA b takes logit row b (row stride ld) and writes token[b]; CTA 0 alone advances.
 __global__ void __launch_bounds__(1024)
-argmax_kernel(const float* __restrict__ logits, int n, int* __restrict__ token, int* advance, int n_advance) {
+argmax_kernel(const float* __restrict__ logits, long long ld, int n, int* __restrict__ token, int* advance,
+              int n_advance) {
   __shared__ float s_v[32];
   __shared__ int s_i[32];
   pdl_trigger();
   pdl_wait();
+  logits += blockIdx.x * ld;
+  token += blockIdx.x;
+  if (blockIdx.x) n_advance = 0;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   float best = -INFINITY;
   int bi = 0x7fffffff;
@@ -414,7 +482,20 @@ extern "C" int dbir_rope_kv(const float* qkv, int64_t ldqkv, int32_t rows, int32
   DBIR_CHECK_CUDA(dbir_launch(rope_kv_kernel, dim3(rows, heads), dim3(HD / 2), 0, ST(stream), qkv,
                               static_cast<long long>(ldqkv), heads, p0, theta, reinterpret_cast<op_t*>(q),
                               static_cast<long long>(ldq), reinterpret_cast<op_t*>(k_cache),
-                              reinterpret_cast<op_t*>(v_cache)));
+                              reinterpret_cast<op_t*>(v_cache), 0LL));
+  return 0;
+}
+
+extern "C" int dbir_rope_kv_seqs(const float* qkv, int64_t ldqkv, int32_t seqs, int32_t heads, const int32_t* p0,
+                                 float theta, void* q, int64_t ldq, void* k_cache, void* v_cache, int64_t cache_stride,
+                                 void* stream) {
+  DBIR_REQUIRE(qkv && p0 && q && k_cache && v_cache && seqs > 0 && heads > 0 && ldqkv >= 3LL * heads * HD &&
+                   ldq >= static_cast<int64_t>(heads) * HD && cache_stride >= static_cast<int64_t>(heads) * HD,
+               "dbir_rope_kv_seqs: bad args");
+  DBIR_CHECK_CUDA(dbir_launch(rope_kv_kernel, dim3(seqs, heads), dim3(HD / 2), 0, ST(stream), qkv,
+                              static_cast<long long>(ldqkv), heads, p0, theta, reinterpret_cast<op_t*>(q),
+                              static_cast<long long>(ldq), reinterpret_cast<op_t*>(k_cache),
+                              reinterpret_cast<op_t*>(v_cache), static_cast<long long>(cache_stride)));
   return 0;
 }
 
@@ -434,50 +515,103 @@ extern "C" int64_t dbir_attention_decode_ws_bytes(int32_t heads, int32_t capacit
   return static_cast<int64_t>(heads) * ((capacity + DEC_CHUNK - 1) / DEC_CHUNK) * (HD + 2) * 4;
 }
 
-extern "C" int dbir_attention_decode(const void* q, const void* k_cache, const void* v_cache, int32_t heads,
-                                     int32_t capacity, const int32_t* len, void* ws, int64_t ws_bytes, void* out,
-                                     void* stream) {
+extern "C" int dbir_attention_decode_seqs(const void* q, int64_t ldq, const void* k_cache, const void* v_cache,
+                                          int64_t cache_stride, int32_t seqs, int32_t heads, int32_t capacity,
+                                          const int32_t* len, void* ws, int64_t ws_bytes, void* out, int64_t ldo,
+                                          void* stream) {
   DBIR_REQUIRE(q && k_cache && v_cache && len && ws && out && heads > 0 && capacity > 0 && al16(q) && al16(k_cache),
                "dbir_attention_decode: bad args");
-  DBIR_REQUIRE(ws_bytes >= dbir_attention_decode_ws_bytes(heads, capacity),
-               "dbir_attention_decode: workspace of %lld bytes, need %lld", (long long)ws_bytes,
-               (long long)dbir_attention_decode_ws_bytes(heads, capacity));
+  DBIR_REQUIRE(seqs > 0 && seqs <= 65535 && (seqs == 1 || (ldq % 8 == 0 && ldq >= static_cast<int64_t>(heads) * HD &&
+                                                           ldo >= static_cast<int64_t>(heads) * HD &&
+                                                           cache_stride % 8 == 0 &&
+                                                           cache_stride >= static_cast<int64_t>(capacity) * heads * HD)),
+               "dbir_attention_decode_seqs: bad batch layout (seqs %d)", seqs);
+  const int64_t need = seqs * dbir_attention_decode_ws_bytes(heads, capacity);
+  DBIR_REQUIRE(ws_bytes >= need, "dbir_attention_decode: workspace of %lld bytes, need %lld", (long long)ws_bytes,
+               (long long)need);
   const int nsplit = (capacity + DEC_CHUNK - 1) / DEC_CHUNK;
-  DBIR_CHECK_CUDA(dbir_launch(attention_decode_part_kernel, dim3(heads, nsplit), dim3(128), 0, ST(stream),
-                              reinterpret_cast<const op_t*>(q), reinterpret_cast<const op_t*>(k_cache),
-                              reinterpret_cast<const op_t*>(v_cache), heads, len, static_cast<float*>(ws)));
-  DBIR_CHECK_CUDA(dbir_launch(attention_decode_combine_kernel, dim3(heads), dim3(HD), 0, ST(stream),
-                              static_cast<const float*>(ws), len, nsplit, reinterpret_cast<op_t*>(out)));
+  DBIR_CHECK_CUDA(dbir_launch(attention_decode_part_kernel, dim3(heads, nsplit, seqs), dim3(128), 0, ST(stream),
+                              reinterpret_cast<const op_t*>(q), static_cast<long long>(ldq),
+                              reinterpret_cast<const op_t*>(k_cache), reinterpret_cast<const op_t*>(v_cache),
+                              static_cast<long long>(cache_stride), heads, len, static_cast<float*>(ws)));
+  DBIR_CHECK_CUDA(dbir_launch(attention_decode_combine_kernel, dim3(heads, seqs), dim3(HD), 0, ST(stream),
+                              static_cast<const float*>(ws), len, nsplit, reinterpret_cast<op_t*>(out),
+                              static_cast<long long>(ldo)));
   return 0;
 }
 
-extern "C" int dbir_gemv(const void* w, int64_t ldw, const void* x, int32_t N, int32_t K, int32_t epilogue,
-                         int32_t pack, const float* residual, void* y, int32_t out_kind, void* stream) {
+extern "C" int dbir_attention_decode(const void* q, const void* k_cache, const void* v_cache, int32_t heads,
+                                     int32_t capacity, const int32_t* len, void* ws, int64_t ws_bytes, void* out,
+                                     void* stream) {
+  return dbir_attention_decode_seqs(q, 0, k_cache, v_cache, 0, 1, heads, capacity, len, ws, ws_bytes, out, 0, stream);
+}
+
+template <int MODE, int R>
+cudaError_t launch_gemv_rows(cudaStream_t st, const op_t* w, long long ldw, const op_t* x, long long ldx, int n_out,
+                             int K, int pack, const float* residual, long long ldr, void* y, long long ldy,
+                             int out_kind) {
+  constexpr int per_cta = GemvShape<MODE, R>::WARPS * GemvShape<MODE, R>::OUTS;
+  return dbir_launch(gemv_kernel<MODE, R>, dim3((n_out + per_cta - 1) / per_cta), dim3(GemvShape<MODE, R>::WARPS * 32),
+                     0, st, w, ldw, x, ldx, n_out, K, pack, residual, ldr, y, ldy, out_kind);
+}
+
+template <int MODE>
+cudaError_t launch_gemv(int M, cudaStream_t st, const op_t* w, long long ldw, const op_t* x, long long ldx, int n_out,
+                        int K, int pack, const float* residual, long long ldr, void* y, long long ldy, int out_kind) {
+#define DBIR_GEMV_ROWS(R)                                                                                    \
+  case R:                                                                                                    \
+    return launch_gemv_rows<MODE, R>(st, w, ldw, x, ldx, n_out, K, pack, residual, ldr, y, ldy, out_kind);
+  switch (M) {
+    DBIR_GEMV_ROWS(1) DBIR_GEMV_ROWS(2) DBIR_GEMV_ROWS(3) DBIR_GEMV_ROWS(4)
+    DBIR_GEMV_ROWS(5) DBIR_GEMV_ROWS(6) DBIR_GEMV_ROWS(7) DBIR_GEMV_ROWS(8)
+    default: return cudaErrorInvalidValue;
+  }
+#undef DBIR_GEMV_ROWS
+}
+
+extern "C" int dbir_gemv_rows(const void* w, int64_t ldw, const void* x, int64_t ldx, int32_t M, int32_t N, int32_t K,
+                              int32_t epilogue, int32_t pack, const float* residual, int64_t ldr, void* y, int64_t ldy,
+                              int32_t out_kind, void* stream) {
   DBIR_REQUIRE(w && x && y && N > 0 && K > 0 && K % 8 == 0 && ldw >= K && ldw % 8 == 0 && al16(w) && al16(x),
                "dbir_gemv: bad args (K and ldw multiples of 8, 16-byte aligned operands)");
+  DBIR_REQUIRE(M >= 1 && M <= 8 && (M == 1 || (ldx >= K && ldx % 8 == 0)), "dbir_gemv_rows: M = %d rows (1 .. 8), ldx %lld",
+               M, static_cast<long long>(ldx));
   DBIR_REQUIRE(epilogue >= 0 && epilogue <= 2 && (out_kind == 0 || out_kind == 1), "dbir_gemv: bad epilogue / out_kind");
   DBIR_REQUIRE(epilogue != 1 || residual, "dbir_gemv: epilogue 1 needs a residual");
   DBIR_REQUIRE(epilogue != 2 || (pack >= 2 && pack % 2 == 0 && N % pack == 0),
                "dbir_gemv: SwiGLU needs the tile width `pack` (even, dividing N)");
   const int n_out = epilogue == 2 ? N / 2 : N;
-  const dim3 grid((n_out + GEMV_WARPS - 1) / GEMV_WARPS), block(GEMV_WARPS * 32);
+  DBIR_REQUIRE(M == 1 || (ldy >= n_out && (epilogue != 1 || ldr >= n_out)), "dbir_gemv_rows: bad ldy / ldr");
   const op_t* wp = reinterpret_cast<const op_t*>(w);
   const op_t* xp = reinterpret_cast<const op_t*>(x);
   const long long l = ldw;
   if (epilogue == 0)
-    DBIR_CHECK_CUDA(dbir_launch(gemv_kernel<0>, grid, block, 0, ST(stream), wp, l, xp, n_out, K, pack, residual, y, out_kind));
+    DBIR_CHECK_CUDA(launch_gemv<0>(M, ST(stream), wp, l, xp, ldx, n_out, K, pack, residual, ldr, y, ldy, out_kind));
   else if (epilogue == 1)
-    DBIR_CHECK_CUDA(dbir_launch(gemv_kernel<1>, grid, block, 0, ST(stream), wp, l, xp, n_out, K, pack, residual, y, out_kind));
+    DBIR_CHECK_CUDA(launch_gemv<1>(M, ST(stream), wp, l, xp, ldx, n_out, K, pack, residual, ldr, y, ldy, out_kind));
   else
-    DBIR_CHECK_CUDA(dbir_launch(gemv_kernel<2>, grid, block, 0, ST(stream), wp, l, xp, n_out, K, pack, residual, y, out_kind));
+    DBIR_CHECK_CUDA(launch_gemv<2>(M, ST(stream), wp, l, xp, ldx, n_out, K, pack, residual, ldr, y, ldy, out_kind));
+  return 0;
+}
+
+extern "C" int dbir_gemv(const void* w, int64_t ldw, const void* x, int32_t N, int32_t K, int32_t epilogue,
+                         int32_t pack, const float* residual, void* y, int32_t out_kind, void* stream) {
+  return dbir_gemv_rows(w, ldw, x, 0, 1, N, K, epilogue, pack, residual, 0, y, 0, out_kind, stream);
+}
+
+extern "C" int dbir_argmax_rows(const float* logits, int64_t ld, int32_t M, int32_t n, int32_t* token, int32_t* advance,
+                                int32_t n_advance, void* stream) {
+  DBIR_REQUIRE(logits && token && n > 0 && M > 0 && (M == 1 || ld >= n) && n_advance >= 0 &&
+                   (n_advance == 0 || advance),
+               "dbir_argmax: bad args");
+  DBIR_CHECK_CUDA(dbir_launch(argmax_kernel, dim3(M), dim3(1024), 0, ST(stream), logits, static_cast<long long>(ld), n,
+                              token, advance, n_advance));
   return 0;
 }
 
 extern "C" int dbir_argmax(const float* logits, int32_t n, int32_t* token, int32_t* advance, int32_t n_advance,
                            void* stream) {
-  DBIR_REQUIRE(logits && token && n > 0 && n_advance >= 0 && (n_advance == 0 || advance), "dbir_argmax: bad args");
-  DBIR_CHECK_CUDA(dbir_launch(argmax_kernel, dim3(1), dim3(1024), 0, ST(stream), logits, n, token, advance, n_advance));
-  return 0;
+  return dbir_argmax_rows(logits, 0, 1, n, token, advance, n_advance, stream);
 }
 
 extern "C" int dbir_embed_gather(const void* table, int32_t vocab, const int32_t* ids, int32_t n, int32_t dim, float* out,

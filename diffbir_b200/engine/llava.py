@@ -15,6 +15,13 @@ llava/model/llava_arch.py, clip_encoder.py, multimodal_projector/builder.py and 
   dbir_attention_decode, lm_head dbir_gemv, dbir_argmax advancing the device position). The GEMV reads the same
   packed weights as the prefill GEMMs: one device copy of every weight. The host reads each token back through a
   pinned copy to stop at EOS.
+- Batched decode (generate_list, up to MAX_SEQS images): every image shares the prompt length, so all sequences sit
+  at the same position at every step. Each image's prefill runs on its own (the graph above) and its KV rows are
+  copied into that sequence's cache; then one CUDA-graph replay per token decodes all of them: dbir_gemv_rows reads
+  each weight row once for every sequence, dbir_rope_kv_seqs / dbir_attention_decode_seqs write and read each
+  sequence's cache, dbir_argmax_rows picks each one's token. Every row's arithmetic is the single-sequence kernels',
+  so each caption has the bits of generate on its image. A sequence that has emitted EOS keeps decoding until the
+  last one stops; its extra tokens are dropped.
 
 The KV cache holds prompt length + max_new_tokens rows. A new image needs no clearing: prefill rewrites rows
 0 .. L-1 and every step attends only to the rows written for this image.
@@ -42,7 +49,30 @@ def swiglu_tile(inter: int) -> int:
     raise ValueError(f"intermediate size {inter}: gate/up rows must tile by 64")
 
 
+class _Seqs:
+    """Buffers and decode graphs of batched decoding; sized for `cap_seqs` sequences, used by any B up to it."""
+
+    def __init__(self, eng: "LlavaEngine", cap_seqs: int):
+        cfg, dev, dt = eng.cfg, eng.dev, eng.dt
+        d, f, H = cfg["hidden"], cfg["intermediate"], cfg["heads"]
+        e = lambda *s, dtype=torch.float32: torch.empty(*s, device=dev, dtype=dtype)  # noqa: E731
+        self.cap_seqs = cap_seqs
+        self.h, self.x16 = e(cap_seqs, d), e(cap_seqs, d, dtype=dt)
+        self.qkv, self.q16, self.att16 = e(cap_seqs, 3 * d), e(cap_seqs, d, dtype=dt), e(cap_seqs, d, dtype=dt)
+        self.gu16 = e(cap_seqs, f, dtype=dt)
+        self.logits = e(cap_seqs, cfg["vocab"])
+        self.tok = torch.zeros(cap_seqs, dtype=torch.int32, device=dev)
+        self.kc = torch.zeros(cfg["layers"], cap_seqs, eng.cap, H, arch.LLAVA_HEAD_DIM, device=dev, dtype=dt)
+        self.vc = torch.zeros_like(self.kc)
+        self.stride = eng.cap * H * arch.LLAVA_HEAD_DIM              # elements between two sequences' caches
+        self.ws = torch.empty(cap_seqs * lib.attention_decode_ws_bytes(H, eng.cap), dtype=torch.uint8, device=dev)
+        self.tok_host = torch.zeros(cap_seqs, dtype=torch.int32, pin_memory=True)
+        self.graphs: Dict[int, torch.cuda.CUDAGraph] = {}
+
+
 class LlavaEngine:
+    MAX_SEQS = 8                                    # most sequences one batched decode step takes (dbir_gemv_rows)
+
     def __init__(self, sd: Dict[str, torch.Tensor], prompt_ids: Sequence[int], cfg: dict = None, device="cuda",
                  max_new_tokens: int = 512):
         """sd: a llava_state_dict (CPU or device tensors). Its entries are popped while they are packed, so weights
@@ -151,6 +181,7 @@ class LlavaEngine:
         self.dec_ws = torch.empty(lib.attention_decode_ws_bytes(H, self.cap), dtype=torch.uint8, device=dev)
         self.tok_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
         self._graphs = None
+        self._seqs: Optional[_Seqs] = None
 
     # ------------------------------------------------------------------ public
     @torch.no_grad()
@@ -174,6 +205,75 @@ class LlavaEngine:
             if t == self.cfg["eos"] or len(out) >= n:
                 return out
             run_step()
+
+    @torch.no_grad()
+    def generate_list(self, xs: Sequence[torch.Tensor], max_new_tokens: Optional[int] = None,
+                      use_graphs: bool = True) -> List[List[int]]:
+        """generate for each of up to MAX_SEQS images, decoded together: list i is what generate(xs[i]) returns."""
+        B = len(xs)
+        if B == 1:
+            return [self.generate(xs[0], use_graphs, max_new_tokens)]
+        n = self.max_new if max_new_tokens is None else min(max_new_tokens, self.max_new)
+        S = self._seq_buffers(B)
+        if use_graphs and B not in S.graphs:
+            # before the prefills: the capture's eager run is a decode step of whatever the buffers hold
+            self.state.copy_(self.state0)
+            S.graphs[B] = self._capture(lambda: self._decode_step_seqs(S, B))
+        self.prefill_seqs(xs, use_graphs)
+        run_step = S.graphs[B].replay if use_graphs else (lambda: self._decode_step_seqs(S, B))
+        out: List[List[int]] = [[] for _ in range(B)]
+        done = [False] * B
+        while True:
+            S.tok_host[:B].copy_(S.tok[:B], non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+            for b in range(B):
+                if not done[b]:
+                    t = int(S.tok_host[b])
+                    out[b].append(t)
+                    done[b] = t == self.cfg["eos"] or len(out[b]) >= n
+            if all(done):
+                return out
+            run_step()
+
+    def _seq_buffers(self, B: int) -> _Seqs:
+        if not 1 <= B <= self.MAX_SEQS:
+            raise ValueError(f"{B} sequences: batched decoding takes 1 .. {self.MAX_SEQS}")
+        if self._seqs is None or self._seqs.cap_seqs < B:
+            self._seqs = None                       # free the smaller buffers (and their graphs) first
+            self._seqs = _Seqs(self, B)
+        return self._seqs
+
+    @torch.no_grad()
+    def prefill_seqs(self, xs: Sequence[torch.Tensor], use_graphs: bool = True) -> _Seqs:
+        """The prefill of each image on its own; its KV rows and first token go to sequence b of the batch buffers.
+        Leaves the shared position / length at the first decode step."""
+        S = self._seq_buffers(len(xs))
+        if use_graphs and self._graphs is None:
+            self._graphs = (self._capture(self._prefill), self._capture(self._decode_step))
+        run_prefill = self._graphs[0].replay if use_graphs else self._prefill
+        L = self.L
+        for b, x in enumerate(xs):
+            assert x.shape == self.img.shape
+            self.img.copy_(x)
+            run_prefill()
+            S.kc[:, b, :L].copy_(self.kc[:, :L])
+            S.vc[:, b, :L].copy_(self.vc[:, :L])
+            S.tok[b:b + 1].copy_(self.tok)
+        return S
+
+    @torch.no_grad()
+    def forced_logits_seqs(self, xs: Sequence[torch.Tensor], tokens: Sequence[Sequence[int]]) -> torch.Tensor:
+        """Teacher forcing of B sequences decoded together (eager): [len(tokens[b]) - 1, B, vocab], row i = sequence b's
+        logits after feeding tokens[b][:i + 1] (rows 1.. of forced_logits on image b)."""
+        B = len(xs)
+        S = self.prefill_seqs(xs, use_graphs=False)
+        rows = []
+        steps = len(tokens[0])
+        for i in range(steps - 1):
+            S.tok[:B].copy_(torch.tensor([int(t[i]) for t in tokens], dtype=torch.int32))
+            self._decode_step_seqs(S, B)
+            rows.append(S.logits[:B].clone())
+        return torch.stack(rows) if rows else torch.empty(0, B, self.cfg["vocab"], device=self.dev)
 
     @torch.no_grad()
     def prefill_logits(self, x: torch.Tensor) -> torch.Tensor:
@@ -284,3 +384,24 @@ class LlavaEngine:
         lib.rmsnorm(h, d, 1, d, W["norm"], x16, d, eps=cfg["rms_eps"])
         lib.gemv(W["lm_head"], x16, self.logits, N=cfg["vocab"], K=d)
         lib.argmax(self.logits, cfg["vocab"], self.tok, advance=self.state)
+
+    def _decode_step_seqs(self, S: _Seqs, B: int):
+        """_decode_step for sequences 0 .. B-1 of S, all at the shared position."""
+        cfg, W = self.cfg, self.w
+        d, f, H, V = cfg["hidden"], cfg["intermediate"], cfg["heads"], cfg["vocab"]
+        h, x16, qkv, q16, att16, gu16 = S.h[:B], S.x16[:B], S.qkv[:B], S.q16[:B], S.att16[:B], S.gu16[:B]
+        lib.embed_gather(W["embed"], V, S.tok, B, d, h, d)
+        for i in range(cfg["layers"]):
+            o = f"l{i}."
+            lib.rmsnorm(h, d, B, d, W[o + "ln1"], x16, d, eps=cfg["rms_eps"])
+            lib.gemv_rows(W[o + "qkv"], x16, qkv, M=B, N=3 * d, K=d, ldx=d, ldy=3 * d)
+            lib.rope_kv_seqs(qkv, 3 * d, B, H, self.state[0:1], q16, d, S.kc[i], S.vc[i], S.stride,
+                             theta=cfg["rope_theta"])
+            lib.attention_decode_seqs(q16, d, S.kc[i], S.vc[i], S.stride, B, H, self.cap, self.state[1:2], S.ws, att16, d)
+            lib.gemv_rows(W[o + "o"], att16, h, M=B, N=d, K=d, ldx=d, ldy=d, epilogue="residual", residual=h, ldr=d)
+            lib.rmsnorm(h, d, B, d, W[o + "ln2"], x16, d, eps=cfg["rms_eps"])
+            lib.gemv_rows(W[o + "gu"], x16, gu16, M=B, N=2 * f, K=d, ldx=d, ldy=f, epilogue="swiglu", pack=self.bn)
+            lib.gemv_rows(W[o + "down"], gu16, h, M=B, N=d, K=f, ldx=f, ldy=d, epilogue="residual", residual=h, ldr=d)
+        lib.rmsnorm(h, d, B, d, W["norm"], x16, d, eps=cfg["rms_eps"])
+        lib.gemv_rows(W["lm_head"], x16, S.logits, M=B, N=V, K=d, ldx=d, ldy=V)
+        lib.argmax_rows(S.logits, V, B, V, S.tok, advance=self.state)

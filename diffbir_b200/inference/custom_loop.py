@@ -13,7 +13,7 @@ from PIL import Image
 
 from ..pipeline import SwinIRPipeline
 from ..utils.common import instantiate_from_config
-from .loop import InferenceLoop, check_supported, load_checkpoint
+from .loop import InferenceLoop, batch_images_setup, check_supported, load_checkpoint
 from .ranks import Ranks
 
 
@@ -22,6 +22,7 @@ class CustomInferenceLoop(InferenceLoop):
         self.args = args
         self.ranks = ranks
         check_supported(args)
+        batch_images_setup(args)
         if not args.train_cfg or not args.ckpt:
             raise ValueError("--version custom needs --train_cfg (the stage-2 training YAML) and --ckpt (ControlNet weights)")
         with open(args.train_cfg) as f:

@@ -9,7 +9,7 @@ import csv
 import os
 from argparse import Namespace
 from pathlib import Path
-from typing import Generator, List, Optional
+from typing import Callable, Generator, Iterable, Iterator, List, Optional, TypeVar
 
 import numpy as np
 import torch
@@ -101,6 +101,50 @@ def check_supported(args: Namespace) -> None:
     # pipeline, which (like the reference) runs un-tiled when the image is smaller than a tile
     if (args.vae_encoder_tiled and args.vae_encoder_tile_size <= 512) or (args.vae_decoder_tiled and args.vae_decoder_tile_size <= 512):
         raise NotImplementedError("Tiled-VAE is outside the path (SURVEY.md §8f); the VAE engines run un-tiled")
+    check_batch_images(args)
+
+
+def check_batch_images(args: Namespace) -> None:
+    """--batch_images N restores up to N inputs of one size per Pipeline.run call. Refused where a call already holds
+    several samples or tiles, or where one input is more than one restoration."""
+    n = getattr(args, "batch_images", 1)
+    if n < 1:
+        raise ValueError(f"--batch_images {n}: must be at least 1")
+    if n == 1:
+        return
+    why = None
+    if args.n_samples > 1:
+        why = "--n_samples > 1 already batches the samples of one input"
+    elif getattr(args, "distribute", "images") == "cooperate":
+        why = "--distribute cooperate puts every GPU on one input at a time; use --distribute images"
+    elif args.task == "unaligned_face":
+        why = "--task unaligned_face restores each face and the background as inputs of their own"
+    elif args.cleaner_tiled or args.cldm_tiled or args.vae_encoder_tiled or args.vae_decoder_tiled:
+        why = "tiled inputs already fill the GPU with tile units (--cleaner_tiled, --cldm_tiled, VAE tiling)"
+    if why:
+        raise NotImplementedError(f"--batch_images {n}: {why}")
+
+
+def batch_images_setup(args: Namespace) -> None:
+    """--batch_images N > 1: pins the batch-invariant kernel plans (as torchrun does), so an image's output does not
+    depend on the other images of its call. Must run before the engines are built."""
+    if getattr(args, "batch_images", 1) > 1:
+        os.environ["DBIR_DETERMINISTIC"] = "1"
+
+
+T = TypeVar("T")
+
+
+def shape_groups(items: Iterable[T], n: int, shape: Callable[[T], tuple]) -> Iterator[List[T]]:
+    """Consecutive runs of at most n items of one shape, in order: a change of shape closes the run."""
+    group: List[T] = []
+    for item in items:
+        if group and (len(group) == n or shape(item) != shape(group[0])):
+            yield group
+            group = []
+        group.append(item)
+    if group:
+        yield group
 
 
 def prompt_with_caption(caption: str, pos_prompt: str) -> str:
@@ -116,6 +160,7 @@ class InferenceLoop:
         self.args = args
         self.ranks = ranks
         check_supported(args)
+        batch_images_setup(args)
         self.loop_ctx = {}
         self.pipeline = None
         self.weights_dir = getattr(args, "weights_dir", None) or default_weights_dir()
@@ -226,6 +271,8 @@ class InferenceLoop:
     @torch.no_grad()
     def run(self) -> None:
         a = self.args
+        if getattr(a, "batch_images", 1) > 1:
+            return self.run_batched()
         self.setup()
         for lq in self.load_lq():
             # fp32 logits; nothing here runs under autocast
@@ -247,6 +294,32 @@ class InferenceLoop:
                 samples.extend(list(batch_samples))
             if self.ranks is None or self.ranks.writes:
                 self.save(samples, pos_prompt, neg_prompt)
+        if self.ranks is not None:
+            self.ranks.finish(self.save_dir)
+
+    @torch.no_grad()
+    def run_batched(self) -> None:
+        """--batch_images N > 1: consecutive inputs of one size after after_load_lq, up to N of them, are captioned
+        together and restored by one Pipeline.run. Image k (its index in the sorted list) draws its noise from
+        generators seeded seed + k, the seed rule of --distribute images, so with the batch-invariant plans its output
+        is the one it gets when restored alone after set_seed(seed + k). Files are written in input order."""
+        a = self.args
+        self.setup()
+        loaded = ((lq, self.after_load_lq(lq), self.loop_ctx["file_stem"], self.loop_ctx["image_index"])
+                  for lq in self.load_lq())
+        for group in shape_groups(loaded, a.batch_images, lambda item: item[1].shape):
+            captions = self.captioner.caption_list([lq for lq, _, _, _ in group])
+            pos_prompts = [prompt_with_caption(c, a.pos_prompt) for c in captions]
+            samples = self.pipeline.run(
+                np.stack([arr for _, arr, _, _ in group]), a.steps, a.strength, a.cleaner_tiled, a.cleaner_tile_size,
+                a.cleaner_tile_stride, a.vae_encoder_tiled, a.vae_encoder_tile_size, a.vae_decoder_tiled,
+                a.vae_decoder_tile_size, a.cldm_tiled, a.cldm_tile_size, a.cldm_tile_stride, pos_prompts, a.neg_prompt,
+                a.cfg_scale, a.start_point_type, a.sampler, a.noise_aug, a.rescale_cfg, a.s_churn, a.s_tmin, a.s_tmax,
+                a.s_noise, a.eta, a.order, seeds=[a.seed + k for _, _, _, k in group])
+            if self.ranks is None or self.ranks.writes:
+                for (_, _, stem, k), sample, pos_prompt in zip(group, samples, pos_prompts):
+                    self.loop_ctx["file_stem"], self.loop_ctx["image_index"] = stem, k
+                    self.save([sample], pos_prompt, a.neg_prompt)
         if self.ranks is not None:
             self.ranks.finish(self.save_dir)
 

@@ -455,6 +455,40 @@ def gemv(w, x, y, *, N, K, ldw=0, epilogue="none", pack=0, residual=None):
     count_launch()
 
 
+def rope_kv_seqs(qkv, ldqkv, seqs, heads, p0, q, ldq, k_cache, v_cache, cache_stride, theta=10000.0):
+    """rope_kv of `seqs` sequences at one position p0[0]: row b writes cache b (cache_stride elements apart)."""
+    check(load().dbir_rope_kv_seqs(_fp(qkv), C.c_int64(ldqkv), seqs, heads, _fp(p0), C.c_float(theta), _fp(q),
+                                   C.c_int64(ldq), _fp(k_cache), _fp(v_cache), C.c_int64(cache_stride), _sp()),
+          "dbir_rope_kv_seqs")
+    count_launch()
+
+
+def attention_decode_seqs(q, ldq, k_cache, v_cache, cache_stride, seqs, heads, capacity, length, ws, out, ldo):
+    """attention_decode of query row b against cache b for b < seqs; ws: seqs x attention_decode_ws_bytes bytes."""
+    check(load().dbir_attention_decode_seqs(_fp(q), C.c_int64(ldq), _fp(k_cache), _fp(v_cache), C.c_int64(cache_stride),
+                                            seqs, heads, capacity, _fp(length), _fp(ws),
+                                            C.c_int64(ws.numel() * ws.element_size()), _fp(out), C.c_int64(ldo), _sp()),
+          "dbir_attention_decode_seqs")
+    count_launch(2)
+
+
+def gemv_rows(w, x, y, *, M, N, K, ldx, ldy, ldw=0, epilogue="none", pack=0, residual=None, ldr=0):
+    """gemv over M <= 8 rows of x (op16 [M, ldx]) -> y [M, ldy]; each weight row is read once for all M rows and
+    every row's bits equal gemv of that row alone."""
+    check(load().dbir_gemv_rows(_fp(w), C.c_int64(ldw or K), _fp(x), C.c_int64(ldx), M, N, K, GEMV_EPILOGUE[epilogue],
+                                pack, _fp(residual), C.c_int64(ldr), _fp(y), C.c_int64(ldy),
+                                0 if y.dtype == torch.float32 else 1, _sp()), "dbir_gemv_rows")
+    count_launch()
+
+
+def argmax_rows(logits, ld, M, n, tokens, advance=None):
+    """argmax of each of M fp32 logit rows [M, ld] -> device int32 tokens [M]; `advance` is incremented once."""
+    n_adv = 0 if advance is None else advance.numel()
+    check(load().dbir_argmax_rows(_fp(logits), C.c_int64(ld), M, n, _fp(tokens), _fp(advance), n_adv, _sp()),
+          "dbir_argmax_rows")
+    count_launch()
+
+
 def argmax(logits, n, token, advance=None):
     """First maximum of fp32 logits [n] -> device int32 token; each element of `advance` (device int32) += 1."""
     n_adv = 0 if advance is None else advance.numel()
@@ -554,6 +588,17 @@ def brownian_increment(out, seed, lo, hi, t0, t1, depth):
     check(load().dbir_brownian_increment(_fp(out), C.c_int64(out.numel()), C.c_uint64(seed), C.c_double(lo),
                                          C.c_double(hi), C.c_double(t0), C.c_double(t1), depth, _sp()),
           "dbir_brownian_increment")
+    count_launch()
+
+
+def brownian_increment_samples(out, seeds, lo, hi, t0, t1, depth):
+    """out (fp32 [B, ...], contiguous, on the device): sample b = brownian_increment of its own slice with seeds[b]
+    (device int64 [B], the uint64 seeds' bits)."""
+    b = out.shape[0]
+    assert seeds.dtype == torch.int64 and seeds.numel() == b and seeds.device == out.device
+    check(load().dbir_brownian_increment_samples(_fp(out), C.c_int64(out.numel() // b), b, _fp(seeds), C.c_double(lo),
+                                                 C.c_double(hi), C.c_double(t0), C.c_double(t1), depth, _sp()),
+          "dbir_brownian_increment_samples")
     count_launch()
 
 

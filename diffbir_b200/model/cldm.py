@@ -240,6 +240,19 @@ class ControlLDM:
         return (dict(c_txt=c_txt[:n].contiguous(), c_img=c_img),
                 dict(c_txt=c_txt[n:].contiguous(), c_img=c_img.clone()))
 
+    @torch.no_grad()
+    def prepare_condition_pairs(self, cond_img: torch.Tensor, pos_txt: List[str], neg_txt: str,
+                                tiled: bool = False, tile_size: int = -1):
+        """prepare_condition_pair with a positive prompt per image. Image i's text rows are what Pipeline.run of that
+        image alone computes on an empty cache: (pos_txt[i], neg_txt) as one text-tower batch of 2. The tower's
+        rows depend on its batch size, so they are neither read from nor written to the per-prompt cache, whose
+        entries may come from batches of another size. A distinct positive prompt is encoded once per call."""
+        self._build()
+        pairs = {p: self.clip(self.tokenize([p, neg_txt])) for p in dict.fromkeys(pos_txt)}
+        c_img = self.vae_encode(cond_img * 2 - 1, sample=False, tiled=tiled, tile_size=tile_size)
+        return (dict(c_txt=torch.stack([pairs[p][0] for p in pos_txt]), c_img=c_img),
+                dict(c_txt=torch.stack([pairs[p][1] for p in pos_txt]), c_img=c_img.clone()))
+
     # --------------------------------------------------------------- denoiser
     @torch.no_grad()
     def forward(self, x_noisy: torch.Tensor, t: torch.Tensor, cond: Dict[str, torch.Tensor]) -> torch.Tensor:

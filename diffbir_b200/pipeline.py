@@ -5,7 +5,7 @@ networks are the kernel engines behind diffbir_b200.model.{SwinIR, ControlLDM}.
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -14,7 +14,7 @@ import torch.nn.functional as F
 from . import lib
 from .model import ControlLDM, Diffusion
 from .sampler import DDIMSampler, DPMSolverSampler, EDMSampler, SpacedSampler
-from .sampler.sampler import tiled_run_chunked
+from .sampler.sampler import NoiseSource, randn, randn_like, tiled_run_chunked
 from .utils.common import make_tiled_fn, sliding_windows, wavelet_reconstruction
 
 
@@ -96,9 +96,21 @@ class Pipeline:
                    vae_decoder_tiled, vae_decoder_tile_size, cldm_tiled, cldm_tile_size,
                    cldm_tile_stride, pos_prompt, neg_prompt, cfg_scale, start_point_type,
                    sampler_type, noise_aug, rescale_cfg, s_churn, s_tmin, s_tmax, s_noise, eta,
-                   order, x_T: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """pipeline.py:71-233."""
+                   order, x_T: Optional[torch.Tensor] = None, seeds: Optional[Sequence[int]] = None) -> torch.Tensor:
+        """pipeline.py:71-233. pos_prompt: one prompt for every image, or one per image. seeds: one per image; image k
+        then draws its noise from its own generators seeded seeds[k] (NoiseSource) instead of the global ones."""
         bs, _, h0, w0 = cond_img.shape
+        source = None
+        if seeds is not None:
+            if len(seeds) != bs:
+                raise ValueError(f"{len(seeds)} seeds for {bs} images")
+            source = NoiseSource(seeds, self.device)
+        if isinstance(pos_prompt, str):
+            pos_prompts = [pos_prompt] * bs
+        else:
+            pos_prompts = list(pos_prompt)
+            if len(pos_prompts) != bs:
+                raise ValueError(f"{len(pos_prompts)} positive prompts for {bs} images")
         cond_img = pad_to_multiples_of(cond_img, multiple=64 if not vae_encoder_tiled and not cldm_tiled else 8)
         vae_encoder_tiled, vae_decoder_tiled = vae_tiling(cond_img.shape[2:], vae_encoder_tiled, vae_encoder_tile_size,
                                                           vae_decoder_tiled, vae_decoder_tile_size)
@@ -112,7 +124,10 @@ class Pipeline:
         # the latent is deterministic (posterior mode), so it is encoded once and shared.
         # Both prompts go through the text tower as one batch (pipeline.py:117-128 runs it twice).
         enc_tiling = dict(tiled=True, tile_size=vae_encoder_tile_size) if vae_encoder_tiled else {}
-        cond, uncond = self.cldm.prepare_condition_pair(cond_img, [pos_prompt] * bs, [neg_prompt] * bs, **enc_tiling)
+        if isinstance(pos_prompt, str):
+            cond, uncond = self.cldm.prepare_condition_pair(cond_img, pos_prompts, [neg_prompt] * bs, **enc_tiling)
+        else:       # image i's text rows as its run alone computes them, whatever else shares the call
+            cond, uncond = self.cldm.prepare_condition_pairs(cond_img, pos_prompts, neg_prompt, **enc_tiling)
         self._mark("encode+clip")
         h1, w1 = cond["c_img"].shape[2:]
         if cldm_tiled and (h1 < cldm_tile_size // 8 or w1 < cldm_tile_size // 8):
@@ -129,13 +144,13 @@ class Pipeline:
                 x_T = self.diffusion.q_sample(
                     cond["c_img"],
                     torch.full((bs,), self.diffusion.num_timesteps - 1, dtype=torch.long, device=self.device),
-                    torch.randn(cond["c_img"].shape, dtype=torch.float32, device=self.device))
+                    randn(cond["c_img"].shape, self.device, source))
             else:
-                x_T = torch.randn((bs, 4, h2, w2), dtype=torch.float32, device=self.device)
+                x_T = randn((bs, 4, h2, w2), self.device, source)
         if noise_aug > 0:
             cond["c_img"] = self.diffusion.q_sample(
                 x_start=cond["c_img"], t=torch.full(size=(bs,), fill_value=noise_aug, device=self.device),
-                noise=torch.randn_like(cond["c_img"]))
+                noise=randn_like(cond["c_img"], source))
             uncond["c_img"] = cond["c_img"].detach().clone()
         control_scales = self.cldm.control_scales
         self.cldm.control_scales = [strength] * 13
@@ -153,6 +168,7 @@ class Pipeline:
         sampler.shard_batch = self.shard_batch
         sampler.shard_tiles = self.shard_tiles
         sampler.max_tile_forwards = self.max_tile_forwards
+        sampler.noise_source = source
         if cldm_tiled and tiled_run_chunked(len(sliding_windows(h2, w2, cldm_tile_size // 8, cldm_tile_stride // 8)),
                                             1 if cfg_scale == 1.0 else 2, bs, self.max_tile_forwards,
                                             sampler.shard_tiles):
@@ -186,11 +202,17 @@ class Pipeline:
     def run(self, lq: np.ndarray, steps: int, strength: float, cleaner_tiled: bool,
             cleaner_tile_size: int, cleaner_tile_stride: int, vae_encoder_tiled: bool,
             vae_encoder_tile_size: int, vae_decoder_tiled: bool, vae_decoder_tile_size: int,
-            cldm_tiled: bool, cldm_tile_size: int, cldm_tile_stride: int, pos_prompt: str,
+            cldm_tiled: bool, cldm_tile_size: int, cldm_tile_stride: int, pos_prompt: Union[str, List[str]],
             neg_prompt: str, cfg_scale: float, start_point_type: str, sampler_type: str,
             noise_aug: int, rescale_cfg: bool, s_churn: float, s_tmin: float, s_tmax: float,
-            s_noise: float, eta: float, order: int, x_T: Optional[torch.Tensor] = None) -> np.ndarray:
-        """pipeline.py:235-321: uint8 [B,H,W,3] (numpy or pinned CPU tensor) -> uint8 numpy."""
+            s_noise: float, eta: float, order: int, x_T: Optional[torch.Tensor] = None,
+            seeds: Optional[Sequence[int]] = None) -> np.ndarray:
+        """pipeline.py:235-321: uint8 [B,H,W,3] (numpy or pinned CPU tensor) -> uint8 numpy.
+
+        pos_prompt: a str for every image (the reference's meaning) or a list of B prompts, one per image.
+        seeds: one per image; every random draw of image k then comes from its own generators seeded seeds[k], in the
+        order the run of that image alone makes after set_seed(seeds[k]) (sampler.NoiseSource). With the
+        batch-invariant kernel plans (DBIR_DETERMINISTIC=1) image k's output is then that run's, bit for bit."""
         host = torch.from_numpy(lq) if isinstance(lq, np.ndarray) else lq
         lq_dev = host.to(self.device, non_blocking=True)                        # H2D
         out = self.run_device(lq_dev, steps, strength, cleaner_tiled, cleaner_tile_size,
@@ -198,7 +220,7 @@ class Pipeline:
                               vae_decoder_tiled, vae_decoder_tile_size, cldm_tiled, cldm_tile_size,
                               cldm_tile_stride, pos_prompt, neg_prompt, cfg_scale, start_point_type,
                               sampler_type, noise_aug, rescale_cfg, s_churn, s_tmin, s_tmax, s_noise,
-                              eta, order, x_T=x_T)
+                              eta, order, x_T=x_T, seeds=seeds)
         return out.cpu().numpy()                                                # D2H
 
     @torch.no_grad()
@@ -206,7 +228,7 @@ class Pipeline:
                    cleaner_tile_stride, vae_encoder_tiled, vae_encoder_tile_size, vae_decoder_tiled,
                    vae_decoder_tile_size, cldm_tiled, cldm_tile_size, cldm_tile_stride, pos_prompt,
                    neg_prompt, cfg_scale, start_point_type, sampler_type, noise_aug, rescale_cfg,
-                   s_churn, s_tmin, s_tmax, s_noise, eta, order, x_T=None) -> torch.Tensor:
+                   s_churn, s_tmin, s_tmax, s_noise, eta, order, x_T=None, seeds=None) -> torch.Tensor:
         """Same as run() with the uint8 NHWC input and output resident on the device."""
         if self.marks is not None:
             self.marks.clear()
@@ -224,7 +246,7 @@ class Pipeline:
                                  vae_decoder_tiled, vae_decoder_tile_size, cldm_tiled, cldm_tile_size,
                                  cldm_tile_stride, pos_prompt, neg_prompt, cfg_scale, start_point_type,
                                  sampler_type, noise_aug, rescale_cfg, s_churn, s_tmin, s_tmax, s_noise,
-                                 eta, order, x_T=x_T)
+                                 eta, order, x_T=x_T, seeds=seeds)
         if tuple(sample.shape[2:]) == tuple(self.output_size) and sample.is_cuda and self.fused_post:
             # no resize (antialiased bicubic at scale 1 is the identity): colour fix + x255 / clamp /
             # truncate + NHWC in one kernel (dbir_wavelet_fix) instead of ~45 full-resolution passes

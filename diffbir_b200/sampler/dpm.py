@@ -20,7 +20,7 @@ from typing import Callable, List, Optional
 import numpy as np
 import torch
 
-from .sampler import EngineEval, Sampler, tiled_callable
+from .sampler import EngineEval, Sampler, randn, tiled_callable
 
 
 def _piecewise_linear(x: torch.Tensor, xp: torch.Tensor, yp: torch.Tensor) -> torch.Tensor:
@@ -199,7 +199,7 @@ class DPMSolverSampler(Sampler):
                tile_size: int = -1, tile_stride: int = -1, x_T: Optional[torch.Tensor] = None,
                progress: bool = True) -> torch.Tensor:
         if x_T is None:
-            x_T = torch.randn(x_size, device=device, dtype=torch.float32)
+            x_T = randn(x_size, device, self.noise_source)
         ns = DiscreteVP(self.betas)
         use_cfg = not (cfg_scale == 1.0 or uncond is None)
         from ..model.cldm import ControlLDM

@@ -22,12 +22,12 @@ distribution and query semantics, not its random stream.
 """
 from __future__ import annotations
 
-from typing import Callable, Dict, Optional, Tuple
+from typing import Callable, Dict, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 
-from .sampler import EngineEval, Sampler, tiled_callable
+from .sampler import EngineEval, NoiseSource, Sampler, randn, randn_like, tiled_callable
 
 
 def _bc(v: torch.Tensor, ndim: int) -> torch.Tensor:
@@ -46,10 +46,11 @@ def _ancestral(sigma_from, sigma_to, eta):
 class _Run:
     """One sampling run: the denoiser, the sigma ladder and the noise source shared by every step rule."""
 
-    def __init__(self, denoise: Callable, x: torch.Tensor, sigmas: torch.Tensor, hp: dict, noise: Optional[Callable]):
-        self.D, self.x, self.sig, self.hp = denoise, x, sigmas, hp
+    def __init__(self, denoise: Callable, x: torch.Tensor, sigmas: torch.Tensor, hp: dict, noise: Optional[Callable],
+                 source: Optional[NoiseSource] = None):
+        self.D, self.x, self.sig, self.hp, self.source = denoise, x, sigmas, hp, source
         self.ones = x.new_ones([x.shape[0]])
-        self.noise = noise if noise is not None else (lambda s0, s1: torch.randn_like(self.x))
+        self.noise = noise if noise is not None else (lambda s0, s1: randn_like(self.x, self.source))
         self.n = len(sigmas) - 1
 
     def den(self, x, sigma):
@@ -64,7 +65,7 @@ class _Run:
         the trajectory. The noise draw happens every step, churn or not, like the reference."""
         hp, s = self.hp, self.sig
         gamma = min(hp["s_churn"] / self.n, 2 ** 0.5 - 1) if hp["s_tmin"] <= s[i] <= hp["s_tmax"] else 0.0
-        eps = torch.randn_like(self.x) * hp["s_noise"]
+        eps = randn_like(self.x, self.source) * hp["s_noise"]
         sigma_hat = s[i] * (gamma + 1)
         if gamma > 0:
             self.x = self.x + eps * (sigma_hat ** 2 - s[i] ** 2) ** 0.5
@@ -310,27 +311,39 @@ class DeviceBrownianTree:
     """torchsde.BrownianTree(lo, zeros_like(x), hi, entropy=seed) as the engine builds it: `tree(t0, t1)` is
     W(t1) - W(t0) for every element of x, computed by one dbir_brownian_increment launch from (seed, node, element)
     alone. No tree is stored: the same query gives the same bits every time, and an element's value does not depend
-    on the size of x."""
+    on the size of x. With a list of seeds, sample b of x has its own tree, seeded seeds[b]: its slice equals the
+    single-seed tree of that slice alone (one dbir_brownian_increment_samples launch)."""
 
-    def __init__(self, x: torch.Tensor, lo, hi, seed: int):
+    def __init__(self, x: torch.Tensor, lo, hi, seed: Union[int, Sequence[int]]):
         if not x.is_cuda:
             raise ValueError("the device Brownian tree of edm_dpm++_sde needs a CUDA latent (install torchsde to "
                              "sample on another device)")
         self.shape, self.device = x.shape, x.device
-        self.lo, self.hi, self.seed = float(lo), float(hi), int(seed)
+        self.lo, self.hi = float(lo), float(hi)
+        if isinstance(seed, int):
+            self.seed, self.seeds = seed, None
+        else:
+            if len(seed) != x.shape[0]:
+                raise ValueError(f"{len(seed)} seeds for a batch of {x.shape[0]} samples")
+            self.seed, self.seeds = None, torch.tensor([int(s) for s in seed], dtype=torch.int64, device=x.device)
         self.depth = brownian_depth(self.lo, self.hi)
 
     def __call__(self, t0, t1) -> torch.Tensor:
         from .. import lib
         out = torch.empty(self.shape, dtype=torch.float32, device=self.device)
-        lib.brownian_increment(out, self.seed, self.lo, self.hi, float(t0), float(t1), self.depth)
+        if self.seeds is None:
+            lib.brownian_increment(out, self.seed, self.lo, self.hi, float(t0), float(t1), self.depth)
+        else:
+            lib.brownian_increment_samples(out, self.seeds, self.lo, self.hi, float(t0), float(t1), self.depth)
         return out
 
 
-def _brownian_noise(x: torch.Tensor, sigmas: torch.Tensor, solver: str) -> Optional[Callable]:
+def _brownian_noise(x: torch.Tensor, sigmas: torch.Tensor, solver: str,
+                    source: Optional[NoiseSource] = None) -> Optional[Callable]:
     """BrownianTreeNoiseSampler(x, sigma_min, sigma_max) (k_diffusion.py:97-120) on torchsde's tree when torchsde is
     there, else on DeviceBrownianTree. The seed comes from the CPU generator, as in k-diffusion; ranks that cooperate
-    on one image are all seeded alike and make the same CPU draws before this one, so they draw the same seed."""
+    on one image are all seeded alike and make the same CPU draws before this one, so they draw the same seed. With a
+    NoiseSource each sample draws its own seed from its own CPU generator and has its own tree."""
     try:
         import torchsde
     except ImportError:
@@ -338,11 +351,16 @@ def _brownian_noise(x: torch.Tensor, sigmas: torch.Tensor, solver: str) -> Optio
             return None                                     # independent N(0, I) draws: same distribution
         torchsde = None
     lo, hi = torch.as_tensor(sigmas[sigmas > 0].min()), torch.as_tensor(sigmas.max())
-    seed = torch.randint(0, 2 ** 63 - 1, []).item()
+    seed = torch.randint(0, 2 ** 63 - 1, []).item() if source is None else source.randint_seeds()
     if torchsde is None:
         tree = DeviceBrownianTree(x, lo, hi, seed)
-    else:
+    elif source is None:
         tree = torchsde.BrownianTree(lo, torch.zeros_like(x), hi, entropy=seed)
+    else:
+        trees = [torchsde.BrownianTree(lo, torch.zeros_like(x[k:k + 1]), hi, entropy=s) for k, s in enumerate(seed)]
+
+        def tree(t0, t1):
+            return torch.cat([tr(t0, t1) for tr in trees])
 
     def sample(s0, s1):
         a, b = torch.as_tensor(s0), torch.as_tensor(s1)
@@ -352,13 +370,14 @@ def _brownian_noise(x: torch.Tensor, sigmas: torch.Tensor, solver: str) -> Optio
 
 
 def run_rule(solver: str, denoise: Callable, x: torch.Tensor, sigmas: torch.Tensor, hp: dict,
-             noise: Optional[Callable] = None) -> torch.Tensor:
+             noise: Optional[Callable] = None, source: Optional[NoiseSource] = None) -> torch.Tensor:
     """Runs one step rule over the sigma ladder. `noise(sigma, sigma_next)` overrides the rule's noise source
-    (the k-diffusion `noise_sampler` argument; tests inject a seeded one)."""
+    (the k-diffusion `noise_sampler` argument; tests inject a seeded one). `source` draws every other random number
+    per sample (None: the global generators)."""
     rule, names, noise_kind = STEP_RULES[solver]
     if noise is None and noise_kind == "brownian":
-        noise = _brownian_noise(x, sigmas, solver)
-    run = _Run(denoise, x, sigmas, {k: hp[k] for k in names}, noise)
+        noise = _brownian_noise(x, sigmas, solver, source)
+    run = _Run(denoise, x, sigmas, {k: hp[k] for k in names}, noise, source)
     for i in range(run.n):
         rule(run, i)
     return run.x
@@ -433,7 +452,7 @@ class EDMSampler(Sampler):
                progress: bool = True) -> torch.Tensor:
         self.make_schedule(steps)
         if x_T is None:
-            x_T = torch.randn(x_size, device=device, dtype=torch.float32)
+            x_T = randn(x_size, device, self.noise_source)
         from ..model.cldm import ControlLDM
         if isinstance(model, ControlLDM):
             use_cfg = not (uncond is None or cfg_scale == 1.0)
@@ -451,4 +470,4 @@ class EDMSampler(Sampler):
             denoiser = self.convert_to_denoiser(fn, cond, uncond, cfg_scale)
         self.sigmas, self.timesteps = self.sigmas.to(dev), self.timesteps.to(dev)
         x = x_T * torch.sqrt(1.0 + self.sigmas[0] ** 2.0)
-        return run_rule(self.solver, denoiser, x, self.sigmas, self.hp)
+        return run_rule(self.solver, denoiser, x, self.sigmas, self.hp, source=self.noise_source)

@@ -13,7 +13,8 @@ When `model` is a diffbir_b200 ControlLDM the loop runs on the kernel engine:
     re-assembled by a single all-gather per step (every rank then blends and updates the same
     full latent with the same RNG stream).
 Noise is drawn with torch.randn_like once per step exactly like the reference
-(spaced_sampler.py:181, ddim_sampler.py:143): the RNG consumption is the reference's. Outputs are
+(spaced_sampler.py:181, ddim_sampler.py:143): the RNG consumption is the reference's. With a NoiseSource set
+(`Sampler.noise_source`), every draw comes per sample from that sample's own generators instead, in the same order. Outputs are
 bit-reproducible across runs and processes in tiled mode and with DBIR_DETERMINISTIC=1 (batch-invariant
 kernel plans); otherwise the timing-based split-K choice of dbir_gemm may differ between processes
 (rounding-level differences).
@@ -29,6 +30,43 @@ import torch
 
 from .. import lib
 from ..utils.common import gaussian_weights, sliding_windows
+
+
+class NoiseSource:
+    """The random draws of one batch, per sample: sample k draws from its own CUDA and CPU torch.Generator seeded
+    seeds[k], in the order a run of that sample alone draws from the global generators right after
+    set_seed(seeds[k]). Each sample's noise is then the same whichever batch it runs in.
+
+    Without a source (None) the pipeline and the samplers draw from the global generators, as the reference does."""
+
+    def __init__(self, seeds, device) -> None:
+        self.seeds = [int(s) for s in seeds]
+        self.device = torch.device(device)
+        self.gpu = [torch.Generator(self.device).manual_seed(s) for s in self.seeds]
+        # on a CPU device one generator serves both kinds of draw, as torch's global CPU generator does
+        self.cpu = self.gpu if self.device.type == "cpu" else [torch.Generator().manual_seed(s) for s in self.seeds]
+
+    def randn(self, shape) -> torch.Tensor:
+        """torch.randn(shape) in fp32 on the source's device, row k from sample k's device generator."""
+        if shape[0] != len(self.gpu):
+            raise ValueError(f"a batch of {shape[0]} samples drawn from a source of {len(self.gpu)} seeds")
+        return torch.cat([torch.randn((1, *shape[1:]), generator=g, device=self.device, dtype=torch.float32)
+                          for g in self.gpu])
+
+    def randn_like(self, x: torch.Tensor) -> torch.Tensor:
+        return self.randn(tuple(x.shape)).to(x.dtype)
+
+    def randint_seeds(self) -> List[int]:
+        """torch.randint(0, 2**63 - 1, []) from each sample's CPU generator (the Brownian tree's seed)."""
+        return [int(torch.randint(0, 2 ** 63 - 1, [], generator=g).item()) for g in self.cpu]
+
+
+def randn_like(x: torch.Tensor, source: Optional[NoiseSource]) -> torch.Tensor:
+    return torch.randn_like(x) if source is None else source.randn_like(x)
+
+
+def randn(shape, device, source: Optional[NoiseSource]) -> torch.Tensor:
+    return torch.randn(shape, device=device, dtype=torch.float32) if source is None else source.randn(shape)
 
 
 def space_timesteps(num_timesteps: int, steps: int) -> np.ndarray:
@@ -372,6 +410,7 @@ class Sampler:
         # than that run as several replays per evaluation, so memory stops growing with the image size; the
         # 49-tile (98-forward) 2048^2 restoration still takes one replay.
         self.max_tile_forwards = 128
+        self.noise_source: Optional[NoiseSource] = None     # per-sample draws (None: the global generators)
         self.last_stats: dict = {}
 
     def get_cfg_scale(self, default_cfg_scale: float, model_t: int) -> float:
@@ -397,7 +436,7 @@ class Sampler:
         self.make_schedule(steps)
         ts, coefs, mode = self._step_coefs()
         if x_T is None:
-            x_T = torch.randn(x_size, device=device, dtype=torch.float32)
+            x_T = randn(x_size, device, self.noise_source)
         from ..model.cldm import ControlLDM
         if isinstance(model, ControlLDM):
             return self._sample_engine(model, ts, coefs, mode, x_T, cond, uncond, cfg_scale, tiled,
@@ -421,7 +460,7 @@ class Sampler:
         self.last_stats = ev.stats
         for it, tab_idx in enumerate(order):
             e_c, e_u = ev.eps(x, it)
-            noise = torch.randn_like(x)
+            noise = randn_like(x, self.noise_source)
             cur_cfg = self.get_cfg_scale(cfg_scale, model_ts[it])
             if cur_cfg == 1.0:
                 e_u = None      # the reference takes the cond-only branch on such steps (spaced_sampler.py:150-152)
@@ -446,7 +485,7 @@ class Sampler:
                 ec, eu = fwd(x, model_t, cond), fwd(x, model_t, uncond)
                 e = eu + s * (ec - eu)
             c = coefs[tab_idx]
-            noise = torch.randn_like(x)
+            noise = randn_like(x, self.noise_source)
             if mode in (0, 1):
                 x0 = c[0] * x - c[1] * e
                 x = (c[2] * x0 + c[3] * x) + c[4] * noise

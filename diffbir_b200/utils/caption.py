@@ -28,6 +28,10 @@ class Captioner:
     def __call__(self, image: Image.Image) -> str:
         raise NotImplementedError
 
+    def caption_list(self, images: List[Image.Image]) -> List[str]:
+        """The caption of each image, each one what __call__ gives for that image alone."""
+        return [self(image) for image in images]
+
 
 class EmptyCaptioner(Captioner):
     def __call__(self, image: Image.Image) -> str:
@@ -89,6 +93,12 @@ class RAMCaptioner(Captioner):
     def __call__(self, image: Image.Image) -> str:
         x = preprocess(image, self.size).to(self.engine.dev)
         return decide(self.engine.forward(x)[0], self.thresholds, self.tags)
+
+    @torch.no_grad()
+    def caption_list(self, images: List[Image.Image]) -> List[str]:
+        """One engine forward over the batch (a graph per batch size)."""
+        x = torch.cat([preprocess(image, self.size) for image in images]).to(self.engine.dev)
+        return [decide(row, self.thresholds, self.tags) for row in self.engine.forward(x)]
 
 
 # ---- LLaVA-1.5-7B (reference utils/caption.py:52-145, --llava_bit 16) -------------------------------------------------
@@ -284,6 +294,16 @@ class LLaVACaptioner(Captioner):
     def __call__(self, image: Image.Image) -> str:
         ids = self.engine.generate(preprocess_llava(image, self.size).to(self.engine.dev))
         return self.tokenizer.decode(ids).strip()
+
+    @torch.no_grad()
+    def caption_list(self, images: List[Image.Image]) -> List[str]:
+        """Greedy decoding of up to LlavaEngine.MAX_SEQS images at a time, each step reading the weights once for all
+        of them; every caption is the one __call__ gives for its image."""
+        out: List[str] = []
+        for i in range(0, len(images), self.engine.MAX_SEQS):
+            xs = [preprocess_llava(image, self.size).to(self.engine.dev) for image in images[i:i + self.engine.MAX_SEQS]]
+            out += [self.tokenizer.decode(ids).strip() for ids in self.engine.generate_list(xs)]
+        return out
 
 
 def llava_bit_message(llava_bit) -> str:

@@ -227,6 +227,15 @@ int dbir_parse_mask(const float* logits, int64_t ld, int64_t rows, int32_t class
  * dbir_argmax: first maximum of fp32 logits [n] -> *token (greedy decoding, temperature 0); then each of
  *   advance[0 .. n_advance-1] (device int32) is incremented by one: the decode step's position and length.
  * dbir_embed_gather: fp32 out[i, ldo] = embed_tokens[ids[i]] (op16 [vocab, dim]; ids device int32 [n]).
+ * Batched decode (B sequences at the same position, each with its own KV cache; every row's bits equal the
+ * single-sequence call on that row):
+ * dbir_rope_kv_seqs: row b of qkv is sequence b at position p0[0]; its k / v go to row p0[0] of cache b, which starts
+ *   cache_stride elements after cache b - 1.
+ * dbir_attention_decode_seqs: query row b (q op16 [B, ldq]) against the first len[0] rows of cache b -> out [B, ldo].
+ *   ws: B * dbir_attention_decode_ws_bytes(heads, capacity) bytes.
+ * dbir_gemv_rows: dbir_gemv over M <= 8 input rows (x op16 [M, ldx], residual / y [M, ldr] / [M, ldy]): each weight
+ *   row is read once for all M inputs; each row's sum runs in the single-row order.
+ * dbir_argmax_rows: dbir_argmax of each of M logit rows [M, ld] -> token[0 .. M-1]; advance is incremented once.
  */
 int dbir_rmsnorm(const float* x, int64_t ldx, int32_t rows, int32_t c, const float* w, float eps, void* out, int64_t ldo,
                  void* stream);
@@ -242,6 +251,16 @@ int dbir_gemv(const void* w, int64_t ldw, const void* x, int32_t N, int32_t K, i
 int dbir_argmax(const float* logits, int32_t n, int32_t* token, int32_t* advance, int32_t n_advance, void* stream);
 int dbir_embed_gather(const void* table, int32_t vocab, const int32_t* ids, int32_t n, int32_t dim, float* out,
                       int64_t ldo, void* stream);
+int dbir_rope_kv_seqs(const float* qkv, int64_t ldqkv, int32_t seqs, int32_t heads, const int32_t* p0, float theta,
+                      void* q, int64_t ldq, void* k_cache, void* v_cache, int64_t cache_stride, void* stream);
+int dbir_attention_decode_seqs(const void* q, int64_t ldq, const void* k_cache, const void* v_cache,
+                               int64_t cache_stride, int32_t seqs, int32_t heads, int32_t capacity, const int32_t* len,
+                               void* ws, int64_t ws_bytes, void* out, int64_t ldo, void* stream);
+int dbir_gemv_rows(const void* w, int64_t ldw, const void* x, int64_t ldx, int32_t M, int32_t N, int32_t K,
+                   int32_t epilogue, int32_t pack, const float* residual, int64_t ldr, void* y, int64_t ldy,
+                   int32_t out_kind, void* stream);
+int dbir_argmax_rows(const float* logits, int64_t ld, int32_t M, int32_t n, int32_t* token, int32_t* advance,
+                     int32_t n_advance, void* stream);
 
 /* ---- small / memory-bound ops ------------------------------------------------------------
  * conv3x3_small_cin : stems with <= 16 input channels; input = virtual concat of two NCHW
@@ -361,6 +380,8 @@ int dbir_pair_nhwc(const float* lq, const float* hq, int32_t b, int32_t c, int64
  *   last level W(t) is one more bridge draw between the leaf's ends, keyed with t. t0 and t1 are clamped to [lo, hi].
  *   Every draw is a Philox4x32-10 normal (Box-Muller) keyed by (seed, node, element); the walk runs in fp64.
  *   0 <= depth <= 62; pick it so that (hi - lo) / 2^depth is the tolerance wanted.
+ * brownian_increment_samples: one tree per sample of a batch: out[b * n + e] (b < samples, e < n) is element e of
+ *   brownian_increment with seed seeds[b] (seeds: device uint64 [samples]), bit for bit.
  * brownian_draws: the raw draws that walk uses, for checking the stream: for e < n, the four Philox words
  *   (words_out uint32 [n, 4]) and the normal (normals fp64 [n]) of element e at `node` (heap numbering: 0 is W(hi),
  *   1 the midpoint of [lo, hi], 2k and 2k + 1 the midpoints of node k's halves), or with leaf = 1 of the leaf draw
@@ -368,6 +389,8 @@ int dbir_pair_nhwc(const float* lq, const float* hq, int32_t b, int32_t c, int64
  */
 int dbir_brownian_increment(float* out, int64_t n, uint64_t seed, double lo, double hi, double t0, double t1,
                             int32_t depth, void* stream);
+int dbir_brownian_increment_samples(float* out, int64_t n, int32_t samples, const uint64_t* seeds, double lo,
+                                    double hi, double t0, double t1, int32_t depth, void* stream);
 int dbir_brownian_draws(uint32_t* words_out, double* normals, int64_t n, uint64_t seed, uint64_t node, int32_t leaf,
                         double t, void* stream);
 

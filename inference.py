@@ -101,6 +101,9 @@ def build_parser() -> ArgumentParser:
     p.add_argument("--distribute", type=str, default="images", choices=["images", "cooperate"],
                    help="Under torchrun: deal the images over the GPUs (images) or run every image on all of them "
                         "(cooperate). Ignored otherwise.")
+    p.add_argument("--batch_images", type=int, default=1,
+                   help="Restore up to N consecutive inputs of one size per call (image k seeded seed + k, as under "
+                        "--distribute images; each output is the one of that image restored alone).")
     return p
 
 
