@@ -113,7 +113,15 @@ class ParseNetEngine:
             out += self._masks(faces[i:i + MAX_BATCH])
         return out
 
+    def masks_device(self, faces: Sequence[np.ndarray]) -> torch.Tensor:
+        """masks as one uint8 [n, 512, 512] tensor on the engine's device (the paste-back's engine path reads it)."""
+        assert all(f.shape == (SIZE, SIZE, 3) and f.dtype == np.uint8 for f in faces)
+        return torch.cat([self._masks_device(faces[i:i + MAX_BATCH]) for i in range(0, len(faces), MAX_BATCH)])
+
     def _masks(self, faces: Sequence[np.ndarray]) -> List[np.ndarray]:
+        return list(self._masks_device(faces).cpu().numpy())
+
+    def _masks_device(self, faces: Sequence[np.ndarray]) -> torch.Tensor:
         n = len(faces)
         src = torch.from_numpy(np.stack(faces)).to(self.dev)
         x16 = self.ws.get("in16", (n * SIZE * SIZE, 3), lib.operand_dtype())
@@ -121,4 +129,4 @@ class ParseNetEngine:
         logits = self.logits(x16, n)
         out = torch.empty(n * SIZE * SIZE, dtype=torch.uint8, device=self.dev)
         lib.parse_mask(logits, self.n_mask, n * SIZE * SIZE, self.classes, out)
-        return list(out.view(n, SIZE, SIZE).cpu().numpy())
+        return out.view(n, SIZE, SIZE)

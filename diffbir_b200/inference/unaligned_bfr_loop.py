@@ -9,6 +9,7 @@ An image without a detected face writes only its prompt.csv row, as in the refer
 from typing import Generator, List
 
 import numpy as np
+import torch
 from PIL import Image
 
 from ..pipeline import BSRNetPipeline, SwinIRPipeline
@@ -54,7 +55,8 @@ class UnAlignedBFRInferenceLoop(InferenceLoop):
         return list(self.pipeline_dict.values())
 
     def face_networks(self):
-        """(detector, parser) callables of FaceRestoreHelper, on the engines."""
+        """(detector, parser) callables of FaceRestoreHelper, on the engines. The parser returns device tensors, so the
+        paste-back runs on the engine too."""
         from .. import arch
         from ..engine.parsenet import ParseNetEngine
         from ..engine.retinaface import RetinaFaceEngine
@@ -66,7 +68,7 @@ class UnAlignedBFRInferenceLoop(InferenceLoop):
             parse_sd = arch.parsenet_state_dict(load_checkpoint(resolve("parsenet", self.weights_dir)))
         det = RetinaFaceEngine(det_sd, device=self.args.device)
         parse = ParseNetEngine(parse_sd, device=self.args.device)
-        return det.candidates, parse.masks
+        return det.candidates, parse.masks_device
 
     def setup(self) -> None:
         import os
@@ -126,6 +128,13 @@ class UnAlignedBFRInferenceLoop(InferenceLoop):
         per_sample = list(map(list, zip(*self.face_samples)))          # [sample k][face i]
         masks = helper.parse_faces([f for faces in per_sample for f in faces])    # one batched parse
         n_faces = len(self.face_samples)
+        if isinstance(masks, torch.Tensor):        # engine masks: every sample pasted on the device in one call
+            for k, (restored, restored_bg) in enumerate(zip(helper.paste_faces_device(samples, per_sample, masks),
+                                                            samples)):
+                file_name = f"{stem}_{k}.png"
+                Image.fromarray(restored_bg).save(os.path.join(self.restored_bg_dir, file_name))
+                Image.fromarray(restored).save(os.path.join(self.save_dir, file_name))
+            return
         for k, (faces, restored_bg) in enumerate(zip(per_sample, samples)):
             for face in faces:
                 helper.add_restored_face(face)

@@ -607,3 +607,50 @@ def brownian_draws(n, seed, node, *, leaf=False, t=0.0, words=None, normals=None
     check(load().dbir_brownian_draws(_fp(words), _fp(normals), C.c_int64(n), C.c_uint64(seed), C.c_uint64(node),
                                      1 if leaf else 0, C.c_double(t), _sp()), "dbir_brownian_draws")
     count_launch()
+
+
+# ---- face paste-back (include/diffbir_b200.h, "face paste-back") ----
+def _map6(m):
+    return (C.c_double * 6)(*[float(v) for v in m])
+
+
+def paste_square(m, face_size, h, w, roi, square, total):
+    """square (fp32 [rh, rw]) = 2x2 erode of the warped ones over roi (x0, y0, rw, rh); total (fp64 [1]) its sum."""
+    x0, y0, rw, rh = roi
+    check(load().dbir_paste_square(_map6(m), face_size, h, w, x0, y0, rw, rh, _fp(square), _fp(total), _sp()),
+          "dbir_paste_square")
+    count_launch()
+
+
+def paste_soft(square, h, w, roi, edge, taps, tmp, soft):
+    x0, y0, rw, rh = roi
+    check(load().dbir_paste_soft(_fp(square), h, w, x0, y0, rw, rh, edge, _fp(taps), _fp(tmp), _fp(soft), _sp()),
+          "dbir_paste_soft")
+    count_launch(4 if edge else 2)
+
+
+def paste_parse_blur(masks, taps, tmp, out):
+    """masks u8 [n, s, s] -> out fp64: two blurs with taps, 10-pixel frame zeroed, / 255."""
+    n, s = masks.shape[0], masks.shape[1]
+    check(load().dbir_paste_parse_blur(_fp(masks), n, s, _fp(taps), taps.numel(), _fp(tmp), _fp(out), _sp()),
+          "dbir_paste_parse_blur")
+    count_launch(4)
+
+
+def paste_compose(faces, pms, square, soft, m, h, w, roi, out):
+    """faces u8 [ns, fs, fs, 3], pms fp64 [ns, fs, fs] (any sample stride), out fp64 [ns, h, w, 3]."""
+    x0, y0, rw, rh = roi
+    check(load().dbir_paste_compose(_fp(faces), C.c_int64(faces.stride(0)), _fp(pms), C.c_int64(pms.stride(0)),
+                                    faces.shape[0], _fp(square), _fp(soft), _map6(m), faces.shape[1], h, w, x0, y0, rw,
+                                    rh, _fp(out), _sp()), "dbir_paste_compose")
+    count_launch()
+
+
+def paste_begin(img, out):
+    check(load().dbir_paste_begin(_fp(img), C.c_int64(img.numel()), _fp(out), _sp()), "dbir_paste_begin")
+    count_launch()
+
+
+def paste_end(x, img):
+    check(load().dbir_paste_end(_fp(x), C.c_int64(x.numel()), _fp(img), _sp()), "dbir_paste_end")
+    count_launch()

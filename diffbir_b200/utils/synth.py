@@ -190,3 +190,34 @@ def synthetic_llava(cfg: dict, seed: int = 1234, device="cuda", lm_head_scale: f
             t = 0.02 * torch.randn(shape, generator=g, device=device)
         sd[key] = t
     return sd
+
+
+def synthetic_paste_scene(side: int, n_faces: int, samples: int = 1, seed: int = 0):
+    """A paste-back scene without the networks: a FaceRestoreHelper on a side x side photo holding n_faces inverse
+    affine matrices (landmarks on the 512 template, scaled and rotated, placed so that faces overlap and some are cut
+    by the frame's edge), plus per sample the restored background, the restored faces and parse masks (ellipses).
+    Returns (helper, backgrounds [samples], faces [samples][n_faces], masks uint8 [samples * n_faces, 512, 512])."""
+    import cv2
+    import numpy as np
+    from .face import FaceRestoreHelper
+    rng = np.random.default_rng(seed)
+    helper = FaceRestoreHelper("cuda", detector=lambda img: None, parser=lambda faces: None)
+    helper.read_image(synthetic_lq(side, side, seed=seed)[0])
+    tmpl = helper.face_template
+    for i in range(n_faces):
+        size = rng.uniform(0.12, 0.25) * side                   # about 250-500 pixels at 2048^2
+        cx, cy = rng.uniform(0.02, 0.98, 2) * side                # some faces cut by the frame's edge
+        t = rng.uniform(-0.5, 0.5)
+        rot = np.array([[np.cos(t), -np.sin(t)], [np.sin(t), np.cos(t)]])
+        lm = (tmpl - 256.0) @ rot.T * (size / 512.0) + [cx, cy] + rng.normal(0, 0.5, (5, 2))
+        m = cv2.estimateAffinePartial2D(lm, tmpl, method=cv2.LMEDS)[0]
+        helper.affine_matrices.append(m)
+    helper.get_inverse_affine()
+    backgrounds = [synthetic_lq(side, side, seed=seed + 1 + k)[0] for k in range(samples)]
+    faces = [[synthetic_lq(512, 512, seed=100 * k + i)[0] for i in range(n_faces)] for k in range(samples)]
+    masks = np.zeros((samples * n_faces, 512, 512), np.uint8)
+    for j in range(samples * n_faces):
+        axes = tuple(int(a) for a in rng.uniform(120, 250, 2))
+        cv2.ellipse(masks[j], (int(rng.uniform(200, 312)), int(rng.uniform(200, 312))), axes, rng.uniform(0, 180), 0,
+                    360, 255, -1)
+    return helper, backgrounds, faces, masks

@@ -394,6 +394,37 @@ int dbir_brownian_increment_samples(float* out, int64_t n, int32_t samples, cons
 int dbir_brownian_draws(uint32_t* words_out, double* normals, int64_t n, uint64_t seed, uint64_t node, int32_t leaf,
                         double t, void* stream);
 
+/* ---- face paste-back (utils/face.py FaceRestoreHelper.paste_faces_to_input_image) ---------------------------
+ * Byte-identical restatement of the cv2 / numpy paste of the unaligned-face loop, one face at a time over a region of
+ * interest (x0, y0, rw, rh) of the h x w frame: a rectangle that holds every pixel where the face's warped square,
+ * soft mask or warped parse mask can be non-zero. ROI buffers are fp32 [rh, rw]; borders are the frame's.
+ * `map` is a HOST pointer to the 6 doubles of the destination -> source map (cv2.warpAffine's inverted matrix).
+ * paste_square: cv2.erode(cv2.warpAffine(ones(fs, fs) f32, inv, (w, h)), 2x2 ones) over the ROI; *sum (device fp64)
+ *   receives the ROI's sum.
+ * paste_soft: cv2.GaussianBlur(cv2.erode(square, (2e)x(2e) ones), (2e+1, 2e+1), 0) over the ROI, taps (device f32
+ *   [2e+1]) = cv2.getGaussianKernel(2e+1, 0, CV_32F). edge 0 or >= 3, w a multiple of 4 (cv2's per-column tap
+ *   order is restated for those). tmp: ROI-sized scratch.
+ * paste_parse_blur: masks u8 [n, size, size] -> out f64: two cv2.GaussianBlur((k, k)) with taps (device f64 [k]),
+ *   the 10-pixel frame zeroed, / 255. tmp: same size as out.
+ * paste_compose: for every sample s < samples, out[s] (f64 [h, w, 3]) = mask * pasted + (1 - mask) * out[s] over the
+ *   ROI, with inv_restored = warpAffine(faces[s] u8 [fs, fs, 3]), pm = warpAffine(pms[s] f64 [fs, fs]),
+ *   pasted = square * inv_restored (f32) and mask = min(pm, soft). faces / pms advance by face_stride / pm_stride
+ *   elements per sample.
+ * paste_begin: out f64 = img u8 (n elements); paste_end: img = astype(uint8) (truncation) of in.
+ */
+int dbir_paste_square(const double* map, int32_t face_size, int32_t h, int32_t w, int32_t x0, int32_t y0, int32_t rw,
+                      int32_t rh, float* square, double* sum, void* stream);
+int dbir_paste_soft(const float* square, int32_t h, int32_t w, int32_t x0, int32_t y0, int32_t rw, int32_t rh,
+                    int32_t edge, const float* taps, float* tmp, float* soft, void* stream);
+int dbir_paste_parse_blur(const uint8_t* masks, int32_t n, int32_t size, const double* taps, int32_t k, double* tmp,
+                          double* out, void* stream);
+int dbir_paste_compose(const uint8_t* faces, int64_t face_stride, const double* pms, int64_t pm_stride,
+                       int32_t samples, const float* square, const float* soft, const double* map, int32_t face_size,
+                       int32_t h, int32_t w, int32_t x0, int32_t y0, int32_t rw, int32_t rh, double* out,
+                       void* stream);
+int dbir_paste_begin(const uint8_t* img, int64_t n, double* out, void* stream);
+int dbir_paste_end(const double* in, int64_t n, uint8_t* img, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
