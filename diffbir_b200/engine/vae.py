@@ -9,10 +9,12 @@ operand of each implicit-GEMM convolution; the mid attention (head_dim = C = 512
 64-wide flash kernel) runs as S = Q K^T (GEMM) -> row softmax -> P V^T (GEMM), with V^T
 produced directly by a transposed GEMM so that every operand stays K-major.
 
-This file states the network once, for the un-tiled and the tiled engine: `VaeWalk` runs a batch through
-the encoder or the decoder as a generator that stops at each GroupNorm and asks its driver for the
-statistics. `VaeEngine` answers at once with the batch's own statistics, inside one CUDA graph per input
-shape; `vae_tiled.TiledVae` merges the statistics of all tiles of an image before any of them goes on.
+This file states the network once, for all three VAE engines: `VaeWalk` runs a batch through the encoder or
+the decoder as a generator that stops at each GroupNorm and asks its driver for the statistics. `VaeEngine`
+answers at once with the batch's own statistics, inside one CUDA graph per input shape; `vae_tiled.TiledVae`
+merges the statistics of all tiles of an image before any of them goes on; `vae_sharded.ShardedVae` runs a band
+of image rows per rank (`vae_sharded.BandWalk`, which overrides the few steps where a band differs from a whole
+image) and merges the statistics of all bands.
 """
 from __future__ import annotations
 
@@ -87,36 +89,21 @@ class VaeEngine:
         """Runs the batch x through `net` (VaeWalk.encoder / .decoder), answering each GroupNorm at once with the
         batch's own statistics: from the partial sums the producing conv's epilogue emitted (dbir_gemm gn_partials
         -> dbir_gn_finalize: no second read of the fp32 tensor); tensors written by other kernels take the
-        stand-alone statistics pass.
-
-        The walk's fp32 activations come from three workspace buffers, so nothing is allocated during graph
-        capture. A buffer is handed out again once the tensor it last held has left the walk's state. Three are
-        enough: the walk allocates only while st holds at most two tensors (a ResnetBlock keeps its input or its
-        shortcut, and conv1's output while conv2's is allocated), and it reads a tensor that has left the state
-        only in launches issued before its next allocation. These three are all the full-resolution fp32
-        memory of the un-tiled VAE, which is what bounds the largest image that runs without tiling."""
+        stand-alone statistics pass. The activations take the walk's three workspace buffers: these are all the
+        full-resolution fp32 memory of the un-tiled VAE, which is what bounds the largest image that runs without
+        tiling."""
         ws, nb = self.ws, x.shape[0]
-        st: Dict[str, torch.Tensor] = {}
-        held = [None] * 3
+        walk = VaeWalk(self, ws, nb)
+        stats = ws.get("gn_stats", (nb * 64,), torch.float32)
 
-        def new(*shape):
-            i = next(i for i, t in enumerate(held) if not any(t is v for v in st.values()))
-            held[i] = ws.get(f"x{i}", shape, torch.float32)
-            return held[i]
-
-        gen = net(VaeWalk(self, st, new, ws, nb), x)
-        stats, answer = ws.get("gn_stats", (nb * 64,), torch.float32), None
-        try:
-            while True:
-                c, h, w, part, slots = gen.send(answer)
-                if part is not None:
-                    lib.gn_finalize(part, slots, c, None, 0, 0, nb, h * w, 1e-6, stats)
-                else:
-                    wsp = ws.get("gn_ws", (lib.gn_workspace_floats(nb, h * w, c),), torch.float32, zero=True)
-                    lib.gn_stats(st["cur"], None, c, 0, nb, h * w, 1e-6, stats, wsp)
-                answer = stats
-        except StopIteration as end:
-            return end.value
+        def answer(c, h, w, part, slots):
+            if part is not None:
+                lib.gn_finalize(part, slots, c, None, 0, 0, nb, h * w, 1e-6, stats)
+            else:
+                wsp = ws.get("gn_ws", (lib.gn_workspace_floats(nb, h * w, c),), torch.float32, zero=True)
+                lib.gn_stats(walk.st["cur"], None, c, 0, nb, h * w, 1e-6, stats, wsp)
+            return stats
+        return walk.run(net, x, answer)
 
     def _scratch(self):
         """Allocator for the quant convs inside the graph: each call hands out a workspace buffer of its own."""
@@ -170,16 +157,46 @@ class VaeWalk:
     (mean, rstd) buffer that dbir_gn_apply reads. A convolution's partial sums are read at the next yield and
     nowhere else, so one workspace buffer holds them all.
 
-    The driver supplies the state `st` (the fp32 activations that live from one GroupNorm to the next: "cur" and,
-    inside a ResnetBlock, the pending residual "res"), new(*shape) for fresh fp32 tensors, and the workspace for
-    the 16-bit operands and scratch. No fp32 activation is held in a local across a yield, and none is read after
-    it has left st and new() was called again: between yields a driver may move the state elsewhere, and new()
-    may hand out the memory of a tensor that is no longer in st. Split-K is off in every GEMM, so an image's bits
-    do not depend on the batch it runs in."""
+    The state `st` holds the fp32 activations that live from one GroupNorm to the next: "cur" and, inside a
+    ResnetBlock, the pending residual "res". new(*shape) supplies fresh fp32 tensors, and the workspace the 16-bit
+    operands and scratch. No fp32 activation is held in a local across a yield, and none is read after it has left
+    st and new() was called again: between yields a driver may move the state elsewhere (it passes its own st and
+    new), and new() may hand out the memory of a tensor that is no longer in st. Split-K is off in every GEMM, so an
+    image's bits do not depend on the batch it runs in.
 
-    def __init__(self, eng: VaeEngine, st: Dict[str, torch.Tensor], new, ws: Workspace, nb: int):
+    The walk runs on whole images. A subclass may run it on other layouts of the rows by overriding the steps where
+    they differ: `_halo`, `_down`, `_up` and `_attend`, and `gn_partials`."""
+
+    gn_partials = True          # convolutions emit GroupNorm partial sums where the GEMM can
+
+    def __init__(self, eng: VaeEngine, ws: Workspace, nb: int, st: Dict[str, torch.Tensor] = None, new=None):
         self.w, self.cfg, self.dev, self.op_dtype = eng.w, eng.cfg, eng.dev, eng.op_dtype
-        self.st, self.new, self.ws, self.nb = st, new, ws, nb
+        self.ws, self.nb = ws, nb
+        self.st = {} if st is None else st
+        self._alloc, self._held = new, [None] * 3
+
+    def new(self, *shape) -> torch.Tensor:
+        """A fresh fp32 tensor from the driver's `new`, else from three workspace buffers, so that nothing is
+        allocated during graph capture. A buffer is handed out again once the tensor it last held has left st. Three
+        are enough: the walk allocates only while st holds at most two tensors (a ResnetBlock keeps its input or its
+        shortcut, and conv1's output while conv2's is allocated), and it reads a tensor that has left the state only
+        in launches issued before its next allocation. (Not a bound method stored on the walk: that cycle would keep
+        the walk, and the workspace buffers its tensors view, alive after a call until the garbage collector runs.)"""
+        if self._alloc is not None:
+            return self._alloc(*shape)
+        i = next(i for i, t in enumerate(self._held) if not any(t is v for v in self.st.values()))
+        self._held[i] = self.ws.get(f"x{i}", shape, torch.float32)
+        return self._held[i]
+
+    def run(self, net, x: torch.Tensor, answer):
+        """Runs x through `net` (VaeWalk.encoder / .decoder) and returns its output, answering each GroupNorm stop
+        with answer(c, h, w, partials, slots): the (mean, rstd) buffer of st["cur"]."""
+        gen, stats = net(self, x), None
+        try:
+            while True:
+                stats = answer(*gen.send(stats))
+        except StopIteration as end:
+            return end.value
 
     @staticmethod
     def stops(cfg: dict, decoder: bool) -> int:
@@ -193,7 +210,8 @@ class VaeWalk:
         `out`: NO_PARTIALS when they are not asked for (`out` feeds a resampling, not a GroupNorm) or the GEMM
         cannot emit them for this image shape."""
         W, nb = self.w, self.nb
-        slots = lib.gemm_gn_slots(h, w) if partials else 0
+        self._halo(a16, h, w, cin)
+        slots = lib.gemm_gn_slots(h, w) if partials and self.gn_partials else 0
         part = self.ws.get("part", (nb * slots * cout * 2,), torch.float32) if slots > 0 else None
         lib.gemm(a16, W[key + ".weight"], out, M=nb * h * w, N=cout, K=9 * cin, bias=W[key + ".bias"],
                  residual=residual, conv=(nb, h, w, cin, 3), split_k=1, gn_partials=part)
@@ -226,17 +244,29 @@ class VaeWalk:
 
     def _attn(self, p, c, h, w, src):
         """AttnBlock (single head over the pixels of each image) — vae.py:232-282 — in place on st["cur"]."""
-        ws, W, nb, hw = self.ws, self.w, self.nb, h * w
-        M = nb * hw
+        ws, W, nb, M = self.ws, self.w, self.nb, self.nb * h * w
         stats = yield (c, h, w) + src
         x = self.st["cur"]
         a16 = ws.get("a16", (M, c), self.op_dtype)
         lib.gn_apply(x, None, c, 0, nb, h, w, stats, W[p + "norm.weight"], W[p + "norm.bias"], a16, norm=True,
                      silu=False)
+        self._attend(p, a16, x, c, h, w)
+        return NO_PARTIALS
+
+    def _attend(self, p, a16, x, c, h, w):
+        """The attention after its GroupNorm: x += proj_out(attention over a16, the normalised x)."""
+        ws, W, M = self.ws, self.w, self.nb * h * w
         qk = ws.get("qk16", (M, 2 * c), self.op_dtype)
         lib.gemm(a16, W[p + "qk.w"], qk, M=M, N=2 * c, K=c, bias=W[p + "qk.b"], split_k=1)
         o16 = ws.get("o16", (M, c), self.op_dtype)
-        rows = min(hw, VaeEngine.attn_rows(hw))
+        self._softmax_av(p, qk, a16, o16, c, h * w, 0, h * w)
+        lib.gemm(o16, W[p + "proj_out.weight"], x, M=M, N=c, K=c, bias=W[p + "proj_out.bias"], residual=x, split_k=1)
+
+    def _softmax_av(self, p, qk, a16, o16, c, hw, q0, nq):
+        """Single-head attention of each image b of hw tokens: queries q0 .. q0 + nq - 1 of qk[b * hw:, :c] over the
+        keys qk[b * hw:(b + 1) * hw, c:] and the values v(a16[b * hw:(b + 1) * hw]), into o16[b * nq:(b + 1) * nq]."""
+        ws, W = self.ws, self.w
+        rows = min(nq, VaeEngine.attn_rows(hw))
         # any token count: the key axis of S, P and V^T is padded to a multiple of 8 (16-byte GEMM rows); the
         # softmax runs over the real keys and the padded columns of P and V^T are zero
         kp = -(-hw // 8) * 8
@@ -244,18 +274,17 @@ class VaeWalk:
         p16 = ws.get("p16", (rows, kp), self.op_dtype)
         vt[:, hw:].zero_()
         p16[:, hw:].zero_()
-        for b in range(nb):
+        for b in range(self.nb):
             lib.gemm(W[p + "v.weight"], a16[b * hw:(b + 1) * hw], vt, M=c, N=hw, K=c, bias=W[p + "v.bias"],
                      bias_per_row=True, ldo=kp, split_k=1)
-            for r0 in range(0, hw, rows):
-                r1 = min(hw, r0 + rows)
+            q = b * hw + q0
+            for r0 in range(0, nq, rows):
+                r1 = min(nq, r0 + rows)
                 s = ws.get("s32", (r1 - r0, kp), torch.float32)
-                lib.gemm(qk[b * hw + r0: b * hw + r1], qk[b * hw:(b + 1) * hw, c:], s, M=r1 - r0, N=hw, K=c,
+                lib.gemm(qk[q + r0: q + r1], qk[b * hw:(b + 1) * hw, c:], s, M=r1 - r0, N=hw, K=c,
                          lda=2 * c, ldb=2 * c, ldo=kp, split_k=1)
                 lib.softmax_rows(s, kp, r1 - r0, hw, float(c) ** -0.5, p16, kp)
-                lib.gemm(p16[:r1 - r0], vt, o16[b * hw + r0: b * hw + r1], M=r1 - r0, N=c, K=kp, split_k=1)
-        lib.gemm(o16, W[p + "proj_out.weight"], x, M=M, N=c, K=c, bias=W[p + "proj_out.bias"], residual=x, split_k=1)
-        return NO_PARTIALS
+                lib.gemm(p16[:r1 - r0], vt, o16[b * nq + r0: b * nq + r1], M=r1 - r0, N=c, K=kp, split_k=1)
 
     def _mid(self, p, c, h, w, src):
         src = yield from self._res(p + "mid.block_1.", c, c, h, w, src)
@@ -280,18 +309,14 @@ class VaeWalk:
                                            partials=not (down and j == nres - 1))
                 c = cout
             if down:
-                ho, wo = h // 2, w // 2
-                col = ws.get("a16", (nb * ho * wo, 9 * c), self.op_dtype)
-                lib.im2col_s2(st["cur"], nb, h, w, c, 0, col)
-                st["cur"] = self.new(nb * ho * wo, c)
-                lib.gemm(col, W[f"{p}down.{lvl}.downsample.conv.weight"], st["cur"], M=nb * ho * wo, N=c, K=9 * c,
-                         bias=W[f"{p}down.{lvl}.downsample.conv.bias"], split_k=1)
-                h, w, src = ho, wo, NO_PARTIALS                   # a plain-mode GEMM emits none
+                h, w = self._down(f"{p}down.{lvl}.downsample.conv", c, h, w)
+                src = NO_PARTIALS                                 # a plain-mode GEMM emits none
         src = yield from self._mid(p, c, h, w, src)
         stats = yield (c, h, w) + src
         a16 = ws.get("a16", (nb * h * w, c), self.op_dtype)
         lib.gn_apply(st.pop("cur"), None, c, 0, nb, h, w, stats, W[p + "norm_out.weight"], W[p + "norm_out.bias"],
                      a16, norm=True, silu=True)
+        self._halo(a16, h, w, c)
         zc2 = 2 * cfg["z_channels"]
         m = self.new(nb, h, w, zc2)
         lib.conv3x3_small_cout(a16, nb, h, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], zc2, m, nchw=False)
@@ -314,16 +339,38 @@ class VaeWalk:
                                            partials=not (lvl != 0 and j == nres))
                 c = cout
             if lvl != 0:
-                up16 = ws.get("a16", (nb * 4 * h * w, c), self.op_dtype)
-                lib.gn_apply(st["cur"], None, c, 0, nb, h, w, None, None, None, up16, norm=False, silu=False, upsample=2)
-                h, w = 2 * h, 2 * w
+                up16, h, w = self._up(c, h, w)
                 st["cur"] = self.new(nb * h * w, c)
                 src = self._conv(up16, f"{p}up.{lvl}.upsample.conv", st["cur"], c, c, h, w)
         stats = yield (c, h, w) + src
         a16 = ws.get("a16", (nb * h * w, c), self.op_dtype)
         lib.gn_apply(st.pop("cur"), None, c, 0, nb, h, w, stats, W[p + "norm_out.weight"], W[p + "norm_out.bias"],
                      a16, norm=True, silu=True)
+        self._halo(a16, h, w, c)
         out = torch.empty(nb, cfg["out_ch"], h, w, dtype=torch.float32, device=self.dev)
         lib.conv3x3_small_cout(a16, nb, h, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], cfg["out_ch"], out,
                                nchw=True)
         return out
+
+    # ------------------------------------------------------------------ the steps that depend on the layout
+    def _halo(self, a16, h, w, c) -> None:
+        """Makes the 16-bit operand a16 [nb * h * w, c] of a 3x3 convolution complete: whole images have nothing
+        outside them but the convolution's zero padding."""
+
+    def _down(self, key, c, h, w):
+        """Downsample (vae.py:51-55: pad (0, 1, 0, 1), stride-2 valid conv) of st["cur"] into a new st["cur"];
+        returns its (h, w)."""
+        nb, ho, wo = self.nb, h // 2, w // 2
+        col = self.ws.get("a16", (nb * ho * wo, 9 * c), self.op_dtype)
+        lib.im2col_s2(self.st["cur"], nb, h, w, c, 0, col)
+        self.st["cur"] = self.new(nb * ho * wo, c)
+        lib.gemm(col, self.w[key + ".weight"], self.st["cur"], M=nb * ho * wo, N=c, K=9 * c, bias=self.w[key + ".bias"],
+                 split_k=1)
+        return ho, wo
+
+    def _up(self, c, h, w):
+        """The operand of the Upsample's conv: st["cur"] repeated 2x2 (nearest), 16-bit; returns it and its (h, w)."""
+        up16 = self.ws.get("a16", (self.nb * 4 * h * w, c), self.op_dtype)
+        lib.gn_apply(self.st["cur"], None, c, 0, self.nb, h, w, None, None, None, up16, norm=False, silu=False,
+                     upsample=2)
+        return up16, 2 * h, 2 * w

@@ -3,7 +3,10 @@
 At 2048^2 the un-tiled VAE (encode 26 + decode 48 TFLOP) is the serial remainder of the 8-GPU tiled run:
 every rank would redo it while the sampler loop shrinks with 1/N. Here each rank owns a horizontal band of
 every activation and the result equals the un-sharded engine's (the reference's un-tiled semantics:
-`AutoencoderKL.encode/decode`, vae.py:526-582 — NOT the approximate per-tile GroupNorm of utils/tilevae):
+`AutoencoderKL.encode/decode`, vae.py:526-582 — NOT the approximate per-tile GroupNorm of utils/tilevae).
+
+The network is stated once, in `vae.VaeWalk`; `ShardedVae` drives that walk over this rank's band, and
+`BandWalk` overrides the few steps where a band differs from a whole image:
 
 * **3x3 convolutions**: a band carries one halo row above and below ([n, hb + 2, W, C]); the rows a conv
   needs from the neighbours are exchanged on its 16-bit input (one small all-gather of the two edge rows
@@ -28,15 +31,89 @@ import torch.nn.functional as F
 
 from .. import lib
 from .common import Workspace
-from .vae import VaeEngine
+from .vae import VaeEngine, VaeWalk
+from .vae_tiled import ProcessGroupGather
+
+
+class BandWalk(VaeWalk):
+    """The walk on this rank's band of every image: fp32 NHWC [nb, hb + 2, w, C], this rank's hb rows with one halo
+    row above and below, so that the walk's h is hb + 2."""
+
+    gn_partials = False         # a conv's partial sums would cover the halo rows
+
+    def __init__(self, eng: VaeEngine, ws: Workspace, nb: int, rank: int, world: int, comm):
+        super().__init__(eng, ws, nb)
+        self.rank, self.world, self.comm = rank, world, comm
+
+    def _exchange(self, band: torch.Tensor) -> None:
+        """band [n, hb + 2, W, C] (any dtype): fills the halo rows 0 and hb + 1 with the neighbours' edge rows
+        (zeros at the image border: the convolution's padding)."""
+        edges = torch.stack([band[:, 1], band[:, -2]], 1)                   # [n, 2, W, C]: first / last own row
+        allr = self.comm.all_gather(edges)                                   # [R, n, 2, W, C]
+        if self.rank > 0:
+            band[:, 0] = allr[self.rank - 1, :, 1]
+        else:
+            band[:, 0].zero_()
+        if self.rank < self.world - 1:
+            band[:, -1] = allr[self.rank + 1, :, 0]
+        else:
+            band[:, -1].zero_()
+
+    def _halo(self, a16, h, w, c) -> None:
+        self._exchange(a16.view(self.nb, h, w, c))
+
+    def _down(self, key, c, h, w):
+        """Output row r reads input rows 2r..2r+2: this rank's own rows plus ONE row of the lower neighbour (zeros
+        at the image bottom). The result fills the new band's own rows; its halo rows wait for the next exchange."""
+        n, hb, ws = self.nb, h - 2, self.ws
+        xb = self.st["cur"].view(n, h, w, c)
+        self._exchange(xb)
+        src = xb[:, 1:].contiguous()                                      # [n, hb + 1, w, c]
+        ho, wo = hb // 2, w // 2
+        col = ws.get("col16", (n * ho * wo, 9 * c), self.op_dtype)
+        lib.im2col_s2(src, n, hb + 1, w, c, 0, col)
+        tmp = ws.get("down_tmp", (n, ho, wo, c), torch.float32)
+        lib.gemm(col, self.w[key + ".weight"], tmp, M=n * ho * wo, N=c, K=9 * c, bias=self.w[key + ".bias"])
+        self.st["cur"] = self.new(n * (ho + 2) * wo, c)
+        self.st["cur"].view(n, ho + 2, wo, c)[:, 1:-1] = tmp
+        return ho + 2, wo
+
+    def _up(self, c, h, w):
+        """The upsampled band's own 2 hb rows and one halo row each side, which the conv's exchange fills."""
+        n, hb = self.nb, h - 2
+        up_all = self.ws.get("up_all", (n, 2 * hb + 4, 2 * w, c), self.op_dtype)
+        lib.gn_apply(self.st["cur"], None, c, 0, n, h, w, None, None, None, up_all, norm=False, silu=False, upsample=2)
+        up16 = self.ws.get("a16", (n, 2 * hb + 2, 2 * w, c), self.op_dtype)
+        up16.copy_(up_all[:, 1:-1])
+        return up16, 2 * hb + 2, 2 * w
+
+    def _attend(self, p, a16, x, c, h, w):
+        """Local queries, keys / values of all ranks; proj_out per image on the band's own rows."""
+        ws, W, n = self.ws, self.w, self.nb
+        lw = (h - 2) * w
+        hw = self.world * lw
+        own = a16.view(n, h, w, c)[:, 1:-1].contiguous()                 # [n, hb, w, c]
+        full = self.comm.all_gather(own).permute(1, 0, 2, 3, 4).reshape(n * hw, c).contiguous()   # global row order
+        qk = ws.get("qk16", (n * hw, 2 * c), self.op_dtype)
+        lib.gemm(full, W[p + "qk.w"], qk, M=n * hw, N=2 * c, K=c, bias=W[p + "qk.b"])
+        o16 = ws.get("o16", (n * lw, c), self.op_dtype)
+        self._softmax_av(p, qk, full, o16, c, hw, self.rank * lw, lw)
+        xb = x.view(n, h, w, c)
+        for b in range(n):
+            xi = xb[b, 1:-1].reshape(lw, c)                                # contiguous interior of image b
+            lib.gemm(o16[b * lw:(b + 1) * lw], W[p + "proj_out.weight"], xi, M=lw, N=c, K=c,
+                     bias=W[p + "proj_out.bias"], residual=xi)
 
 
 class ShardedVae:
-    def __init__(self, base: VaeEngine):
-        self.base, self.w, self.cfg, self.dev = base, base.w, base.cfg, base.dev
-        self.op_dtype = base.op_dtype
+    def __init__(self, base: VaeEngine, rank: int = None, world: int = None, comm=None):
+        """Rank `rank` of `world` cooperating ranks (default: the torch.distributed ones) that all call with the same
+        input; `comm.all_gather` (default: `ProcessGroupGather`) carries every exchange between them."""
+        self.base, self.w, self.dev = base, base.w, base.dev
         self.ws = Workspace(self.dev)
-        self.world, self.rank = dist.get_world_size(), dist.get_rank()
+        self.rank = dist.get_rank() if rank is None else rank
+        self.world = dist.get_world_size() if world is None else world
+        self.comm = ProcessGroupGather() if comm is None else comm
 
     # ------------------------------------------------------------------ applicability
     @staticmethod
@@ -48,185 +125,45 @@ class ShardedVae:
         world = dist.get_world_size()
         return h_img % (8 * world) == 0 and h_img // (8 * world) >= 2 and w_img % 8 == 0
 
-    # ------------------------------------------------------------------ collectives
-    def _gather(self, t: torch.Tensor) -> torch.Tensor:
-        out = torch.empty((self.world,) + tuple(t.shape), dtype=t.dtype, device=t.device)
-        dist.all_gather_into_tensor(out, t.contiguous())
-        return out
-
-    def _exchange(self, band: torch.Tensor) -> None:
-        """band [n, hb + 2, W, C] (any dtype): fills the halo rows 0 and hb + 1 with the neighbours' edge rows
-        (zeros at the image border: the convolution's padding)."""
-        edges = torch.stack([band[:, 1], band[:, -2]], 1)                   # [n, 2, W, C]: first / last own row
-        allr = self._gather(edges)                                           # [R, n, 2, W, C]
-        if self.rank > 0:
-            band[:, 0] = allr[self.rank - 1, :, 1]
-        else:
-            band[:, 0].zero_()
-        if self.rank < self.world - 1:
-            band[:, -1] = allr[self.rank + 1, :, 0]
-        else:
-            band[:, -1].zero_()
-
+    # ------------------------------------------------------------------ the driver
     def _gn_stats(self, x: torch.Tensor, n: int, c: int, eps: float) -> torch.Tensor:
         """x fp32 [n, hb + 2, W, c] -> (mean, rstd) of the FULL image per (image, group): stats [n*32*2]."""
         cpg = c // 32
         own = x.view(n, x.shape[1], x.shape[2], 32, cpg)[:, 1:-1]            # this rank's rows (strided view, no copy)
         var, mean = torch.var_mean(own, dim=(1, 2, 4), unbiased=False)       # [n, 32] each
-        both = self._gather(torch.stack([mean, var], -1).double())           # [R, n, 32, 2]
+        both = self.comm.all_gather(torch.stack([mean, var], -1).double())   # [R, n, 32, 2]
         gmean = both[..., 0].mean(0)
         gvar = both[..., 1].mean(0) + (both[..., 0] - gmean).pow(2).mean(0)  # equal counts per rank
         return torch.stack([gmean, (gvar + eps).rsqrt()], -1).float().reshape(-1).contiguous()
 
-    # ------------------------------------------------------------------ blocks on bands
-    def _gn(self, x, c, n, hb, w, gamma, beta, out16, silu, out_raw=None, exchange=True):
-        stats = self._gn_stats(x.view(n, hb + 2, w, c), n, c, 1e-6)
-        lib.gn_apply(x, None, c, 0, n, hb + 2, w, stats, gamma, beta, out16, norm=True, silu=silu, out_raw=out_raw)
-        if exchange:
-            self._exchange(out16.view(n, hb + 2, w, c))
+    def _run(self, net, x: torch.Tensor) -> torch.Tensor:
+        """x fp32 NCHW: the whole input -> `net` (VaeWalk.encoder / .decoder) on this rank's band of its rows."""
+        n, hb = x.shape[0], x.shape[2] // self.world
+        band = F.pad(x, (0, 0, 1, 1))[:, :, self.rank * hb: self.rank * hb + hb + 2].contiguous()   # zero outside
+        walk = BandWalk(self.base, self.ws, n, self.rank, self.world, self.comm)
 
-    def _res(self, p, x, cin, cout, n, hb, w, out):
-        """ResnetBlock.forward (temb None, vae.py:97-117) on a band; out may alias x when cin == cout."""
-        ws, W = self.ws, self.w
-        M = n * (hb + 2) * w
-        a16 = ws.get("a16", (M, cin), self.op_dtype)
-        raw = ws.get("raw16", (M, cin), self.op_dtype) if cin != cout else None
-        self._gn(x, cin, n, hb, w, W[p + "norm1.weight"], W[p + "norm1.bias"], a16, True, raw)
-        h1 = ws.get("h1", (M, cout), torch.float32)
-        lib.gemm(a16, W[p + "conv1.weight"], h1, M=M, N=cout, K=9 * cin, bias=W[p + "conv1.bias"], conv=(n, hb + 2, w, cin, 3))
-        b16 = ws.get("b16", (M, cout), self.op_dtype)
-        self._gn(h1, cout, n, hb, w, W[p + "norm2.weight"], W[p + "norm2.bias"], b16, True)
-        res = x
-        if cin != cout:
-            res = ws.get("skip", (M, cout), torch.float32)
-            lib.gemm(raw, W[p + "nin_shortcut.weight"], res, M=M, N=cout, K=cin, bias=W[p + "nin_shortcut.bias"])
-        lib.gemm(b16, W[p + "conv2.weight"], out, M=M, N=cout, K=9 * cout, bias=W[p + "conv2.bias"], residual=res,
-                 conv=(n, hb + 2, w, cout, 3))
+        def answer(c, h, w, part, slots):                                   # no partial sums on a band
+            return self._gn_stats(walk.st["cur"].view(n, h, w, c), n, c, 1e-6)
+        return walk.run(net, band, answer)
 
-    def _attn(self, p, x, c, n, hb, w):
-        """AttnBlock (vae.py:232-282) in place on the band x: local queries, keys / values of all ranks."""
-        ws, W, R = self.ws, self.w, self.world
-        M = n * (hb + 2) * w
-        a16 = ws.get("a16", (M, c), self.op_dtype)
-        self._gn(x, c, n, hb, w, W[p + "norm.weight"], W[p + "norm.bias"], a16, False, exchange=False)
-        own = a16.view(n, hb + 2, w, c)[:, 1:-1].contiguous()                 # [n, hb, w, c]
-        full = self._gather(own).permute(1, 0, 2, 3, 4).reshape(n, R * hb * w, c).contiguous()   # global row order
-        hw, lw = R * hb * w, hb * w
-        qk = ws.get("qk16", (n * hw, 2 * c), self.op_dtype)
-        lib.gemm(full.view(n * hw, c), W[p + "qk.w"], qk, M=n * hw, N=2 * c, K=c, bias=W[p + "qk.b"])
-        xb = x.view(n, hb + 2, w, c)
-        rows = min(lw, 8192)
-        for b in range(n):
-            vt = ws.get("vt16", (c, hw), self.op_dtype)                       # V^T [C, hw]
-            lib.gemm(W[p + "v.weight"], full[b], vt, M=c, N=hw, K=c, bias=W[p + "v.bias"], bias_per_row=True)
-            o16 = ws.get("o16", (lw, c), self.op_dtype)
-            q0 = b * hw + self.rank * lw                                      # this rank's query rows of image b
-            for r0 in range(0, lw, rows):
-                r1 = min(lw, r0 + rows)
-                s = ws.get("s32", (r1 - r0, hw), torch.float32)
-                lib.gemm(qk[q0 + r0: q0 + r1], qk[b * hw:(b + 1) * hw, c:], s, M=r1 - r0, N=hw, K=c, lda=2 * c, ldb=2 * c)
-                p16 = ws.get("p16", (r1 - r0, hw), self.op_dtype)
-                lib.softmax_rows(s, hw, r1 - r0, hw, float(c) ** -0.5, p16, hw)
-                lib.gemm(p16, vt, o16[r0:r1], M=r1 - r0, N=c, K=hw)
-            xi = xb[b, 1:-1].reshape(lw, c)                                    # contiguous interior of image b
-            lib.gemm(o16, W[p + "proj_out.weight"], xi, M=lw, N=c, K=c, bias=W[p + "proj_out.bias"], residual=xi)
+    def _new(self, *shape) -> torch.Tensor:
+        return torch.empty(*shape, dtype=torch.float32, device=self.dev)
 
-    # ------------------------------------------------------------------ decode
     @torch.no_grad()
     def decode(self, z: torch.Tensor) -> torch.Tensor:
         """z fp32 NCHW [n, 4, h, w] (already divided by the scale factor; identical on every rank) -> image fp32
         NCHW [n, 3, 8h, 8w] on every rank."""
-        cfg, ws, W, R, rk = self.cfg, self.ws, self.w, self.world, self.rank
-        n, zc, h, w = z.shape
-        ch, mult, nres = cfg["ch"], tuple(cfg["ch_mult"]), cfg["num_res_blocks"]
-        hb = h // R
-        # post_quant_conv on the whole (tiny) latent, then this rank's rows + one halo row (zero outside the image)
-        z_nhwc = torch.empty(n * h * w, zc, device=self.dev)
-        lib.nchw_to_nhwc(z, n, zc, h * w, z_nhwc)
-        z2 = torch.empty_like(z_nhwc)
-        lib.linear_f32(z_nhwc, zc, n * h * w, zc, W["post_quant_conv.weight"], W["post_quant_conv.bias"], zc, z2, zc)
-        z2n = torch.empty(n, zc, h, w, device=self.dev)
-        lib.nhwc_to_nchw(z2, n, zc, h * w, z2n)
-        zb = F.pad(z2n, (0, 0, 1, 1))[:, :, rk * hb: rk * hb + hb + 2].contiguous()
-        p = "decoder."
-        c = ch * mult[-1]
-        x = ws.get("x0", (n * (hb + 2) * w, c), torch.float32)
-        lib.conv3x3_small_cin(zb, None, zc, 0, n, hb + 2, w, W[p + "conv_in.weight"], W[p + "conv_in.bias"], c, x)
-        self._res(p + "mid.block_1.", x, c, c, n, hb, w, x)
-        self._attn(p + "mid.attn_1.", x, c, n, hb, w)
-        self._res(p + "mid.block_2.", x, c, c, n, hb, w, x)
-        cur, flip = x, 0
-        for lvl in reversed(range(len(mult))):
-            cout = ch * mult[lvl]
-            for j in range(nres + 1):
-                o = ws.get(f"x{1 + flip}", (n * (hb + 2) * w, cout), torch.float32)
-                self._res(f"{p}up.{lvl}.block.{j}.", cur, c, cout, n, hb, w, o)
-                cur, c, flip = o, cout, flip ^ 1
-            if lvl != 0:
-                up_all = ws.get("up_all", (n, 2 * hb + 4, 2 * w, c), self.op_dtype)
-                lib.gn_apply(cur, None, c, 0, n, hb + 2, w, None, None, None, up_all, norm=False, silu=False, upsample=2)
-                hb, w = 2 * hb, 2 * w
-                up16 = ws.get("a16", (n, hb + 2, w, c), self.op_dtype)
-                up16.copy_(up_all[:, 1:-1])                                   # 2 hb own rows + one halo row each side
-                self._exchange(up16)
-                o = ws.get(f"x{1 + flip}", (n * (hb + 2) * w, c), torch.float32)
-                lib.gemm(up16, W[f"{p}up.{lvl}.upsample.conv.weight"], o, M=n * (hb + 2) * w, N=c, K=9 * c,
-                         bias=W[f"{p}up.{lvl}.upsample.conv.bias"], conv=(n, hb + 2, w, c, 3))
-                cur, flip = o, flip ^ 1
-        a16 = ws.get("a16", (n * (hb + 2) * w, c), self.op_dtype)
-        self._gn(cur, c, n, hb, w, W[p + "norm_out.weight"], W[p + "norm_out.bias"], a16, True)
-        band = torch.empty(n, cfg["out_ch"], hb + 2, w, dtype=torch.float32, device=self.dev)
-        lib.conv3x3_small_cout(a16, n, hb + 2, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], cfg["out_ch"], band,
-                               nchw=True)
-        allb = self._gather(band[:, :, 1:-1].contiguous())                    # [R, n, 3, hb, w]
-        return allb.permute(1, 2, 0, 3, 4).reshape(n, cfg["out_ch"], R * hb, w).contiguous()
+        band = self._run(VaeWalk.decoder, self.base.post_quant(z, self._new))   # post_quant_conv on the whole latent
+        n, oc, _, w = band.shape
+        allb = self.comm.all_gather(band[:, :, 1:-1].contiguous())           # [R, n, 3, hb, w]
+        return allb.permute(1, 2, 0, 3, 4).reshape(n, oc, -1, w).contiguous()
 
-    # ------------------------------------------------------------------ encode
     @torch.no_grad()
     def encode_moments(self, img: torch.Tensor) -> torch.Tensor:
         """img fp32 NCHW [n, 3, H, W] in [-1, 1] (identical on every rank) -> moments fp32 NCHW [n, 8, H/8, W/8]."""
-        cfg, ws, W, R, rk = self.cfg, self.ws, self.w, self.world, self.rank
-        n, ic, h, w = img.shape
-        ch, mult, nres = cfg["ch"], tuple(cfg["ch_mult"]), cfg["num_res_blocks"]
-        hb = h // R
-        p = "encoder."
-        c = ch
-        ib = F.pad(img, (0, 0, 1, 1))[:, :, rk * hb: rk * hb + hb + 2].contiguous()
-        cur = ws.get("x0", (n * (hb + 2) * w, c), torch.float32)
-        lib.conv3x3_small_cin(ib, None, ic, 0, n, hb + 2, w, W[p + "conv_in.weight"], W[p + "conv_in.bias"], c, cur)
-        flip = 0
-        for lvl in range(len(mult)):
-            cout = ch * mult[lvl]
-            for j in range(nres):
-                o = ws.get(f"x{1 + flip}", (n * (hb + 2) * w, cout), torch.float32)
-                self._res(f"{p}down.{lvl}.block.{j}.", cur, c, cout, n, hb, w, o)
-                cur, c, flip = o, cout, flip ^ 1
-            if lvl != len(mult) - 1:
-                # Downsample (vae.py:51-55): pad (0,1,0,1) + stride-2 valid conv. Output row r reads input rows
-                # 2r..2r+2: this rank's own rows plus ONE row of the lower neighbour (zeros at the image bottom).
-                xb = cur.view(n, hb + 2, w, c)
-                self._exchange(xb)
-                src = xb[:, 1:].contiguous()                                  # [n, hb + 1, w, c]
-                ho, wo = hb // 2, w // 2
-                col = ws.get("col16", (n * ho * wo, 9 * c), self.op_dtype)
-                lib.im2col_s2(src, n, hb + 1, w, c, 0, col)
-                tmp = ws.get("down_tmp", (n, ho, wo, c), torch.float32)
-                lib.gemm(col, W[f"{p}down.{lvl}.downsample.conv.weight"], tmp, M=n * ho * wo, N=c, K=9 * c,
-                         bias=W[f"{p}down.{lvl}.downsample.conv.bias"])
-                hb, w = ho, wo
-                o = ws.get(f"x{1 + flip}", (n * (hb + 2) * w, c), torch.float32)
-                o.view(n, hb + 2, w, c)[:, 1:-1] = tmp
-                cur, flip = o, flip ^ 1
-        self._res(p + "mid.block_1.", cur, c, c, n, hb, w, cur)
-        self._attn(p + "mid.attn_1.", cur, c, n, hb, w)
-        self._res(p + "mid.block_2.", cur, c, c, n, hb, w, cur)
-        a16 = ws.get("a16", (n * (hb + 2) * w, c), self.op_dtype)
-        self._gn(cur, c, n, hb, w, W[p + "norm_out.weight"], W[p + "norm_out.bias"], a16, True)
-        zc2 = 2 * cfg["z_channels"]
-        m_band = torch.empty(n * (hb + 2) * w, zc2, dtype=torch.float32, device=self.dev)
-        lib.conv3x3_small_cout(a16, n, hb + 2, w, c, W[p + "conv_out.weight"], W[p + "conv_out.bias"], zc2, m_band, nchw=False)
-        q = torch.empty_like(m_band)
-        lib.linear_f32(m_band, zc2, n * (hb + 2) * w, zc2, W["quant_conv.weight"], W["quant_conv.bias"], zc2, q, zc2)
-        own = q.view(n, hb + 2, w, zc2)[:, 1:-1].contiguous()                 # [n, hb, w, 8]
-        allq = self._gather(own)                                              # [R, n, hb, w, 8]
-        return allq.permute(1, 4, 0, 2, 3).reshape(n, zc2, R * hb, w).contiguous()
+        m = self._run(VaeWalk.encoder, img)                                  # NHWC [n, hb + 2, w, 8]
+        n, hb2, w, zc2 = m.shape
+        q = torch.empty_like(m)
+        lib.linear_f32(m, zc2, n * hb2 * w, zc2, self.w["quant_conv.weight"], self.w["quant_conv.bias"], zc2, q, zc2)
+        allq = self.comm.all_gather(q[:, 1:-1].contiguous())                 # [R, n, hb, w, 8]
+        return allq.permute(1, 4, 0, 2, 3).reshape(n, zc2, -1, w).contiguous()

@@ -436,7 +436,7 @@ class TiledVae:
     def _tiles(self, wv: _Wave, plan: TilePlan, src: torch.Tensor, res: torch.Tensor, decoder: bool):
         """The wave's tiles through VaeWalk: gathered as one NCHW batch, tile-major (entry = tile * N + image), and
         each tile's output cropped to its box of `res` (NCHW for the decoder, NHWC for the encoder)."""
-        walk = VaeWalk(self.base, wv.st, self._new, self.ws, wv.nb)
+        walk = VaeWalk(self.base, self.ws, wv.nb, wv.st, self._new)
         boxes = [plan.in_boxes[t] for t in wv.tiles]
         out = yield from (walk.decoder if decoder else walk.encoder)(
             torch.cat([src[:, :, y0:y1, x0:x1] for x0, x1, y0, y1 in boxes], 0).contiguous())

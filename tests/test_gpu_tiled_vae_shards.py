@@ -1,8 +1,6 @@
 """-m gpu, one device: the tiled VAE sharded over R emulated ranks in one process. R TiledVae instances share one
 VaeEngine, each with its own rank, workspace and a communicator of threads that meet at a barrier; every rank's
 output must be bit-identical to the single-rank TiledVae's, and each rank's last_stats must show its share."""
-import threading
-
 import numpy as np
 import pytest
 import torch
@@ -10,58 +8,22 @@ import torch
 from diffbir_b200 import arch
 from diffbir_b200.utils.synth import make_state_dict
 from tests import tilevae_oracle as otv
-from tests.gpu_util import no_tf32
+from tests.gpu_util import no_tf32, run_ranks
 from tests.small_cfg import VAE_SMALL
 
 pytestmark = pytest.mark.gpu
 
 
-class _Hub:
-    """all_gather among threads: each rank leaves its tensor and waits for the others; the gathered copy is taken
-    on the device's default stream, which every thread launches on, so it follows every rank's writes. A failing
-    rank aborts the barrier and the timeout bounds a wait, so a fault cannot hang the test."""
-
-    def __init__(self, world: int, timeout: float = 300.0):
-        self.bar = threading.Barrier(world, timeout=timeout)
-        self.sent = [None] * world
-
-    def comm(self, rank: int):
-        hub = self
-
-        class _Comm:
-            def all_gather(self, t):
-                hub.sent[rank] = t
-                hub.bar.wait()
-                out = torch.stack(hub.sent, 0)
-                hub.bar.wait()                   # nobody replaces its tensor before every rank has copied
-                return out
-        return _Comm()
-
-
 def _sharded(base, world, method, x, tile, budget=None):
     from diffbir_b200.engine.vae_tiled import TiledVae
-    hub = _Hub(world)
-    tvs = [TiledVae(base, r, world, hub.comm(r)) for r in range(world)]
-    outs, stats, errs = [None] * world, [None] * world, []
 
-    def run(r):
-        try:
-            tvs[r].state_budget = budget
-            outs[r] = getattr(tvs[r], method)(x, tile)
-            stats[r] = dict(tvs[r].last_stats)
-        except BaseException as e:              # noqa: BLE001 -- reported below
-            errs.append((r, e))
-            hub.bar.abort()
+    def run(r, comm):
+        tv = TiledVae(base, r, world, comm)
+        tv.state_budget = budget
+        return getattr(tv, method)(x, tile), dict(tv.last_stats)
 
-    threads = [threading.Thread(target=run, args=(r,)) for r in range(world)]
-    for t in threads:
-        t.start()
-    for t in threads:
-        t.join(timeout=600)
-    torch.cuda.synchronize()
-    assert not errs, errs
-    assert not any(t.is_alive() for t in threads)
-    return outs, stats
+    res, _ = run_ranks(world, run)
+    return [out for out, _ in res], [st for _, st in res]
 
 
 def _expected_share(plan, world, n_img, decoder, wave_pixels):
